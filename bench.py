@@ -1,20 +1,24 @@
 #!/usr/bin/env python
-"""bench.py — ToonCrafter_512 hot path on B200: frames/sec at 320x512x16 frames, DDIM-50, CFG 7.5.
+"""bench.py — ToonCrafter_512 hot path on H100: frames/sec at 320x512x16 frames, DDIM-50, CFG 7.5.
 
 One "step" = one clip: DDIMSampler.sample (50 DDIM steps, cond + uncond UNet evaluation per step) followed by the
 two dual-reference VAE decodes of scripts/evaluation/inference.py:262-270 (T = 16, then T = 14).  Weights are
 seeded synthetic (no checkpoint / network here), inputs synthetic of the reference's shapes.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--ddim-steps 50] [--impl reference]
-                    [--config clip|decode|pair10] [--clips-per-step B]
+                    [--config clip|decode|pair10] [--clips-per-step B] [--dump-outputs DIR]
 
---config clip   (default, BASELINE configs[1]/[2]/[4]) the step described above;
---config decode (configs[3]) step = the two decodes only;
---config pair10 (configs[0]) step = VAE-encode the reference's first 320x512 prompt pair (tests/golden fixture) +
+--config clip   (default) the step described above;
+--config decode step = the two decodes only;
+--config pair10 step = VAE-encode the reference's first 320x512 prompt pair (tests/golden fixture) +
                 DDIM-10 + the two decodes — the configuration the CPU reference is quoted on.
 
+--dump-outputs DIR writes the videos the last timed step returned (float32, stacked over the step's clips) as
+DIR/video.npy.  Every step re-seeds the torch RNG per clip (the DDIM noise), so with the same arguments two builds can
+be compared output for output.
+
 N > 1 is launched by torchrun (one process per GPU, shared-nothing clips, one NCCL weight broadcast at init).
-Prints ONE JSON line (rank 0).  See DESIGN.md §Measurement for every field.
+Prints ONE JSON line (rank 0).
 """
 from __future__ import annotations
 
@@ -33,7 +37,7 @@ ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
-UNET_TF = 12.603                      # TFLOP per UNet forward per sample (SURVEY §8d, matmul/conv, 2 flops/MAC)
+UNET_TF = 12.603                      # TFLOP per UNet forward per sample
 DEC_TF = {16: 37.875, 14: 33.148}     # TFLOP per decode pass
 H, W, T = 40, 64, 16                  # latent geometry of 320x512, 16 frames
 
@@ -48,11 +52,11 @@ def load_peaks():
         d = json.loads(p.read_text())
         return dict(tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 1590.0))), hbm=float(d["hbm_gbs"]),
                     src="measured (MEASURED_PEAKS.json, sustained cuBLAS bf16)")
-    return dict(tflops=1400.0, hbm=6650.0, src="fallback (B200_PROFILING.md)")
+    return dict(tflops=989.0, hbm=3350.0, src="data sheet (H100 SXM: dense fp16 989 TFLOP/s, HBM3 3.35 TB/s at 700 W)")
 
 
 class ClockSampler:
-    """nvidia-smi clock / throttle sampling during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clock / throttle sampling during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -117,7 +121,7 @@ def build_model(dev, rank, world):
                 prm.copy_(synthetic.synthetic_tensor(k, tuple(prm.shape), 0).to(dev))
         if world > 1:
             from tooncrafter_b200.distributed import broadcast_parameters
-            # ONE broadcast of the weights at init (SURVEY §8e); no collective on the data path afterwards
+            # ONE broadcast of the weights at init; no collective on the data path afterwards
             broadcast_parameters(m, src=0)
     m.perframe_ae = True
     return m.eval()
@@ -182,7 +186,7 @@ def workload_config(S, config="clip", clips_per_step=1):
     return {"config": config, "clips_per_gpu_per_step": clips_per_step, "workload": "ToonCrafter_512 320x512x16f DDIM-%d fp16, CFG 7.5 (cond+uncond batched), eta 1.0, "
                         "uniform_trailing, guidance_rescale 0.7, sample() + decode T=16 + decode T=14; "
                         "1 clip per GPU per step; random-init weights, synthetic inputs" % S,
-            "l2": "working set per clip (2.9 GB fp16 weights + activations) exceeds the 126 MB L2",
+            "l2": "working set per clip (2.9 GB fp16 weights + activations) exceeds the 50 MB L2",
             "baseline_note": "vs_baseline = value / 0.667 frames/s (README.md:222: ~24 s/clip on A100)"}
 
 
@@ -219,17 +223,20 @@ def gemm_roofline(model, dev):
 
 
 # ---------------------------------------------------------------------------------------------------- CPU arm
-def gemm_traffic():
-    """(dram bytes per tc_gemm_kernel launch, provenance) from the committed ncu launch list, or (None, reason)."""
-    prof = Path(__file__).resolve().parent / "profiles"
-    p = prof / "r02_unet_b2_launches.gemm_traffic.json"
-    if not p.exists():
-        p = prof / "r01_unet_b2_launches_final.gemm_traffic.json"
-    try:
-        d = json.loads(p.read_text())
-        return float(d["dram_bytes_per_launch"]), f"profiles/{p.name}: {d['launches']} launches, {d['source']}"
-    except Exception as e:      # noqa: BLE001 - the file is optional evidence, not a dependency of the measurement
-        return None, f"no ncu capture committed ({type(e).__name__})"
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_videos(out_dir, videos):
+    """--dump-outputs: the videos the last timed step returned, stacked [clips, 3, T, 320, 512] in float32, as
+    out_dir/video.npy; above 64 MB every k-th element of the flattened stack instead, as out_dir/video_every<k>.npy."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    v = torch.stack([x[0] for x in videos]).float().cpu().numpy()
+    if v.nbytes <= DUMP_LIMIT_BYTES:
+        np.save(os.path.join(out_dir, "video.npy"), v)
+    else:
+        k = -(-v.nbytes // DUMP_LIMIT_BYTES)
+        np.save(os.path.join(out_dir, f"video_every{k}.npy"), np.ascontiguousarray(v.reshape(-1)[::k]))
 
 
 def cpu_threads():
@@ -242,10 +249,10 @@ CPU_ARM_CACHE = ROOT / "gpurun_out" / "cpu_reference_arm.json"
 
 
 def reference_source():
-    """Which implementation the CPU arm executes.  The reference is pure Python without setup.py / pyproject.toml, so
-    `pip install --target baseline/_ref /root/reference` fails ("not installable", DESIGN.md §5) and /root/reference does
-    not exist on the GPU box: unless someone placed an importable copy under baseline/_ref (looked for here), the arm
-    runs the oracle port — the same algorithm, pinned to the reference by the committed goldens."""
+    """Which implementation the CPU arm executes.  The original project is pure Python without setup.py /
+    pyproject.toml, so it cannot be pip-installed: unless an importable copy sits under baseline/_ref
+    (looked for here), the arm runs the oracle port — the same algorithm, pinned to the original by the committed
+    goldens."""
     ref = ROOT / "baseline" / "_ref"
     if (ref / "lvdm" / "models" / "ddpm3d.py").exists():
         return "reference", str(ref)
@@ -340,7 +347,7 @@ def reference_arm(args):
 
 
 def cpu_baseline_for_main_arm(S):
-    """cpu_baseline of the B200 line: the reference arm's measurement when it ran on THIS box within the last hour (the
+    """cpu_baseline of the main line: the reference arm's measurement when it ran on THIS box within the last hour (the
     driver runs it immediately before), otherwise one fresh bounded sample (one UNet forward + one decode)."""
     try:
         d = json.loads(CPU_ARM_CACHE.read_text())
@@ -367,7 +374,7 @@ def cpu_baseline_for_main_arm(S):
 def library_baseline(model, di, fs, S, roof):
     """The reference ALGORITHM on this same GPU through stock PyTorch kernels (cuDNN conv, cuBLAS GEMM, SDPA flash
     attention) under torch.autocast(fp16) with fp32 parameters — what scripts/evaluation/inference.py:323 executes with
-    xformers installed.  This is the number a user gets for free from PyTorch on a B200, i.e. the one to beat.
+    xformers installed.  This is the number a user gets for free from PyTorch on the same GPU, i.e. the one to beat.
     One DDIM step = two B = 1 UNet forwards (ddim.py:221-222); plus the T = 16 and T = 14 decodes."""
     from oracle import unet_oracle, vae_oracle
     from tiny_config import FULL_DDCONFIG, FULL_UNET
@@ -459,7 +466,7 @@ def library_baseline(model, di, fs, S, roof):
 
 # ---------------------------------------------------------------------------------------------------- main
 def pair_inputs(model, dev, S):
-    """BASELINE config #1 inputs: the reference's first 512_interp prompt pair (tests/golden/prompt_pair_74906.npz, made
+    """--config pair10 inputs: the reference's first 512_interp prompt pair (tests/golden/prompt_pair_74906.npz, made
     by tests/golden/make_prompt_pair.py with the transform of inference.py:65-69) as a pinned uint8 host buffer."""
     import numpy as np
     f = np.load(ROOT / "tests" / "golden" / "prompt_pair_74906.npz")["frames"]          # [2, 320, 512, 3] uint8
@@ -467,9 +474,9 @@ def pair_inputs(model, dev, S):
 
 
 def run_pair(model, sampler, frames_u8_host, di, S, fs, dev):
-    """Config #1 through the public API: frames -> first_stage_model.encode(return_hidden_states=True) -> c_concat and
+    """--config pair10 through the public API: frames -> first_stage_model.encode(return_hidden_states=True) -> c_concat and
     ref_context (inference.py:164-200) -> sample(S) -> both decodes.  Only the two DISTINCT frames are encoded (the
-    reference encodes 8 copies of each, SURVEY 8f-1); text / image embeddings are synthetic (no CLIP weights here)."""
+    reference encodes 8 copies of each); text / image embeddings are synthetic (no CLIP weights here)."""
     fr = frames_u8_host.to(dev, non_blocking=True).permute(0, 3, 1, 2).float() / 127.5 - 1.0      # [2, 3, 320, 512]
     post, hidden = model.first_stage_model.encode(fr, return_hidden_states=True)
     z2 = model.get_first_stage_encoding(post)                                                     # [2, 4, 40, 64]
@@ -499,13 +506,15 @@ def main():
     ap.add_argument("--ddim-steps", type=int, default=None, help="default 50 (10 for --config pair10)")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--config", default="clip", choices=["clip", "decode", "pair10"],
-                    help="clip: sample() + both decodes (BASELINE configs 2/3/5); decode: both decodes only (config 4); "
-                         "pair10: encode the reference's prompt pair + DDIM-10 + decodes (config 1)")
+                    help="clip: sample() + both decodes; decode: both decodes only; "
+                         "pair10: encode the reference's prompt pair + DDIM-10 + decodes")
     ap.add_argument("--clips-per-step", type=int, default=1,
                     help="B independent clips per GPU per step, run back to back (B > 1 = B independent B = 1 runs, "
-                         "SURVEY 8e: the reference's decoder is only defined for one clip per call)")
+                         "the reference's decoder is only defined for one clip per call)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-library-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the videos of the last timed step as DIR/video.npy (float32)")
     ap.add_argument("--latency-mode", action="store_true",
                     help="pairs of GPUs share one clip: each evaluates one classifier-free-guidance branch per step "
                          "(one NCCL all-gather per step) and one of the two decodes; needs an even --gpus >= 2")
@@ -549,17 +558,18 @@ def main():
     frames_host = pair_inputs(model, dev, S) if args.config == "pair10" else None
     torch.cuda.synchronize()
 
-    def one_step(inputs):
-        """One step of the selected config on device-resident `inputs` (list of per-clip dicts); returns the last video."""
-        v = None
-        for dj in inputs:
+    def one_step(clips):
+        """One step of the selected config on `clips`, a list of (clip id, device-resident inputs); returns the videos."""
+        videos = []
+        for c, dj in clips:
+            torch.manual_seed(clip_seed(7, c))             # the clip's DDIM noise stream: identical in every step and run
             if args.config == "clip":
-                v = run_clip(model, sampler, dj, S, fs)
+                videos.append(run_clip(model, sampler, dj, S, fs))
             elif args.config == "decode":
-                v = run_decode(model, dj["z"], dj["ref"])
+                videos.append(run_decode(model, dj["z"], dj["ref"]))
             else:
-                v = run_pair(model, sampler, frames_host, dj, S, fs, dev)
-        return v
+                videos.append(run_pair(model, sampler, frames_host, dj, S, fs, dev))
+        return videos
 
     if args.config == "decode":
         for hj, dj in zip(his, dis):
@@ -581,7 +591,7 @@ def main():
 
     # ---- warm-up (builds plans, captures graphs) ------------------------------------------------------------
     for _ in range(max(args.warmup, 1)):
-        one_step(dis)
+        one_step(list(zip(my_clips, dis)))
     barrier()
 
     # ---- timed: device-resident inputs ----------------------------------------------------------------------
@@ -592,10 +602,12 @@ def main():
     barrier()
     e0.record()
     for _ in range(args.steps):
-        one_step(dis)
+        last = one_step(list(zip(my_clips, dis)))
     e1.record()
     barrier()
     ms_dev = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == 0:
+        dump_videos(args.dump_outputs, last)
     clk = clocks.stop() if rank == 0 else None
 
     # ---- timed: end to end through the public API with HOST buffers -----------------------------------------
@@ -616,9 +628,9 @@ def main():
     barrier()
     e0.record()
     for _ in range(args.steps):
-        for hj in his:
+        for c, hj in zip(my_clips, his):
             dj = step_h2d(hj)                              # H2D of this clip's inputs from pinned memory
-            video = one_step([dj])
+            video = one_step([(c, dj)])[0]
             out_host[:, :, :video.shape[2]].copy_(video, non_blocking=True)   # D2H of the clip (latency mode: pair-rank 1
                                                                               # holds the 14-frame variant)
     e1.record()
@@ -690,11 +702,9 @@ def main():
         "clocks": clk,
     }
     if roof is not None:
-        out["roofline"] = {"bound": "tensor", "kernel": "tc_gemm_kernel (implicit-GEMM conv / linear, tcgen05)",
+        out["roofline"] = {"bound": "tensor", "kernel": "tc_gemm_kernel (implicit-GEMM conv / linear, wgmma)",
                            "achieved": roof["tflops"], "peak": peaks["tflops"], "unit": "TFLOP/s",
-                           "frac": roof["tflops"] / peaks["tflops"], "traffic": gemm_traffic()[0],
-                           "traffic_unit": "bytes of DRAM read+write per launch (ncu, average over the GEMM launches of one UNet forward)",
-                           "traffic_source": gemm_traffic()[1], "peak_source": peaks["src"],
+                           "frac": roof["tflops"] / peaks["tflops"], "peak_source": peaks["src"],
                            "launches_per_unet_forward": roof["launches"], "avg_launch_us": roof["avg_launch_us"],
                            "flops_per_launch": roof["flops_per_launch"],
                            "share_of_unet_forward": roof["gemm_ms_per_forward"]}

@@ -1,8 +1,8 @@
-/* tooncrafter_b200 — C ABI of the B200-native DDIM/UNet/VAE-decoder hot path.
+/* tooncrafter_b200 — C ABI of the H100-native DDIM/UNet/VAE-decoder hot path.
  *
  * The reference (Doubiiu/ToonCrafter) has no FFI: its "plugin" seam is Python-object instantiation
  * (utils/utils.py:27-34) and every kernel is a torch library call.  This header is therefore the
- * boundary SURVEY.md §8(b) "B2" asks for: the entry points our Python mirror of lvdm.* calls instead of
+ * boundary: the entry points our Python mirror of lvdm.* calls instead of
  * torch.nn.functional.  Each entry cites the reference call site(s) it replaces.
  *
  * Conventions
@@ -42,7 +42,7 @@ unsigned long long tc_launch_count(void);
 int tc_sm_count(void);
 
 /* ------------------------------------------------------------------------------------------------
- * Implicit-GEMM convolution / linear layer on the tcgen05 tensor cores (TMA-fed, TMEM accumulators).
+ * Implicit-GEMM convolution / linear layer on the Hopper tensor cores (wgmma, TMA-fed, register accumulators).
  *
  *   out[m, j] = epilogue( sum_{tap, c} A[n + dn[tap], y + dy[tap], x + dx[tap], c] * Wt[j, tap*C + c] )
  *
@@ -107,13 +107,13 @@ typedef struct {
 #define TC_GEMM_WS_TICKET_BYTES (64 * 1024) /* head of the workspace: per-tile tickets (4 bytes each) */
 
 int tc_conv_gemm(const TcConvGemm* desc, void* stream);
-/* profiling aids, honoured by trace builds only (TC_BUILD_TRACE=1): mode bits 1 = epilogue skips global stores, 2 = epilogue body skipped (results are then garbage),
- * 4 = record clock64() stamps per CTA / tile / warp role: [160 CTAs][32 tiles][16 slots] read back with *_read_gemm_trace */
+/* profiling aid: bits 8..11 of mode cap the k-slices of later tc_conv_gemm launches (0 = heuristic); other bits are ignored */
 int tc_debug_set_gemm_mode(int mode);
-/* tests: {block_n, cta pair, k-slices, pipeline stages} of the calling thread's process' most recent tc_conv_gemm launch */
+/* tests: {block_n, cta pair (always 0), k-slices, pipeline stages} of the process' most recent tc_conv_gemm launch */
 int tc_debug_last_gemm_config(int* out4);
+/* kept for ABI compatibility: the GEMM kernel records no timeline, so this returns TC_ERR_INVALID */
 int tc_debug_read_gemm_trace(unsigned long long* host_dst, int count);
-/* trace builds only: clock64() stamps of tc_attn3_kernel's CTA (0,0,0), [24 key blocks][16 slots] (scripts/trace_attn.py) */
+/* kept for ABI compatibility: the attention kernel records no timeline, so this returns TC_ERR_INVALID */
 int tc_debug_read_attn_trace(unsigned long long* host_dst, int count);
 
 /* ------------------------------------------------------------------------------------------------
@@ -138,7 +138,7 @@ int tc_layernorm(const void* x, long long ldx, void* y, long long ldy, const flo
                  int rows, int C, float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention, head dim 64, on tcgen05 (QK^T and PV), online softmax in fp32.
+ * Fused attention, head dim 64, on mma.sync tensor-core MMAs (QK^T and PV), online softmax in fp32.
  * q:  [q_batches][Lq][heads*64] (row stride ldq), kv segment s: k/v [kv_batches_s][Lk_s][heads*64].
  * Query batch b attends to kv batch b / kv_div[s].  With two segments the two softmax-attention
  * results are summed (text + image cross attention, attention.py:128-142,153-207); with one it is plain
@@ -170,7 +170,7 @@ int tc_attention_wide(const void* q, const void* k, const void* v, long long ldq
 int tc_softmax_rows(void* s, long long lds, int rows, int cols, float scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Data-movement / elementwise helpers (reference: rearrange/cat/interpolate sites, SURVEY K11)
+ * Data-movement / elementwise helpers (reference: rearrange/cat/interpolate sites)
  */
 /* NCTHW fp32 (B,Cin,T,H,W) -> channels-last fp16 [B][T][H][W][Cpad], zero-padded channels, written at channel
  * offset `coff` of a Cpad-wide tensor (used twice to realise cat([x, c_concat], dim=1), ddpm3d.py:1260-1262);

@@ -4,7 +4,7 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl refere
 under oracle/.  The product path (tooncrafter_b200/) never does.
 
 The reference cannot travel to the GPU box (it only exists in the authoring container), so this module is used
-to (a) validate oracle/ against the real reference and (b) generate tests/golden/ fixtures.  Shims (SURVEY §8c):
+to (a) validate oracle/ against the real reference and (b) generate tests/golden/ fixtures.  Shims:
   1. stub `pytorch_lightning` (ddpm3d.py:21-22, autoencoder.py:7 only need LightningModule/rank_zero_only);
   2. fake `xformers.ops.memory_efficient_attention` backed by F.scaled_dot_product_attention
      (autoencoder_dualref.py:190,316,326 call it unconditionally); installed AFTER lvdm.modules.attention is

@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE ONLY — CPU fp32 restatement of the image-conditioning Resampler (SURVEY 8f-2).
+"""TEST INFRASTRUCTURE ONLY — CPU fp32 restatement of the image-conditioning Resampler.
 
 Follows lvdm/modules/encoders/resampler.py of the reference: Resampler.forward :132-145 (latents repeated per sample,
 proj_in, depth x [PerceiverAttention + latents, FeedForward + latents], proj_out, norm_out), PerceiverAttention.forward

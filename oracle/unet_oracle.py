@@ -74,7 +74,7 @@ def res_block(p: SD, x, emb, B, temporal_conv=True):
 # "einsum": the explicit softmax(q k^T) v of CrossAttention.forward (the numerics oracle: fp32 softmax, fixed op order).
 # "sdpa":   F.scaled_dot_product_attention = what CrossAttention.efficient_forward (attention.py:146-209, xformers
 #           installed) amounts to on a GPU: fused flash kernels, no materialised scores.  Only bench.py's library
-#           baseline switches to it (the fair "best library path" to beat, SURVEY 8c).
+#           baseline switches to it (the fair "best library path" to beat).
 ATTENTION_IMPL = "einsum"
 
 

@@ -58,7 +58,7 @@ def fusion_attention(p: SD, x, ctx, heads=8):
     h = group_norm(x, p.sub("norm."), 1e-6).flatten(2).transpose(1, 2)        # n (hw) c
     q = F.linear(h, p("to_q.weight"))
     b, cc, l, ch, cw = ctx.shape
-    assert b == 1, "reference semantics are only defined for one clip per decode call (SURVEY App. C.3)"
+    assert b == 1, "reference semantics are only defined for one clip per decode call"
     c2 = ctx.permute(0, 2, 3, 4, 1).reshape(1, l * ch * cw, cc)                # [ref0 tokens ; ref1 tokens]
     k = F.linear(c2, p("to_k.weight")).expand(n, -1, -1)
     v = F.linear(c2, p("to_v.weight")).expand(n, -1, -1)
@@ -118,7 +118,7 @@ def decode_first_stage(sd, lay, z, ref_context, scale_factor=0.18215, chunk=16,
                        prefix="first_stage_model.decoder."):
     """ddpm3d.py:647-683 (decode_core, perframe_ae=True): z [1, 4, T, h, w] -> [1, 3, T, 8h, 8w]."""
     b, c, t, hh, ww = z.shape
-    assert b == 1, "B > 1 is defined as B independent B = 1 runs (SURVEY §8e)"
+    assert b == 1, "B > 1 is defined as B independent B = 1 runs"
     zz = z.permute(0, 2, 1, 3, 4).reshape(b * t, c, hh, ww) * (1.0 / scale_factor)
     outs = [decode(sd, lay, zz[i:i + chunk], ref_context, prefix) for i in range(0, zz.shape[0], chunk)]
     out = torch.cat(outs, dim=0)

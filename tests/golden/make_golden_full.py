@@ -3,7 +3,7 @@ authoring container (CPU, fp32, ~10 min, peak RSS ~20 GB):
 
     python tests/golden/make_golden_full.py
 
-What is pinned (BASELINE configs #2 / #4 geometry: inference_512_v1.0 UNet + VAE, T = 16, latent 40 x 64):
+What is pinned (the benchmark geometry: inference_512_v1.0 UNet + VAE, T = 16, latent 40 x 64):
   * three teacher-forced DDIM steps of the reference's own `DDIMSampler.p_sample_ddim` (ddim.py:206-279) at
     S = 50 indices 49 (first, t = 999), 25 (middle) and 0 (last, the sqrt(5.96e-8) step), CFG 7.5, rescale 0.7,
     eta 1: the two UNet outputs (cond / uncond = the B = 2 program the bench times), x_prev and pred_x0;

@@ -1,4 +1,4 @@
-"""Golden for the multi-condition sampler (SURVEY 8f-3): the UNMODIFIED reference
+"""Golden for the multi-condition sampler: the UNMODIFIED reference
 lvdm/models/samplers/ddim_multiplecond.py::DDIMSampler on the tiny configuration, 4 teacher-forced steps, three-way
 guidance (cfg 7.5, cfg_img 4.0, guidance_rescale 0.7) — run in the authoring container:
 

@@ -4,7 +4,7 @@ The engines record flat lists of `tooncrafter_b200.ops.*` calls (tensor, geometr
 every op a plain-PyTorch meaning (fp32 math, fp16 storage) so that the HOST logic — weight packing, buffer
 slicing, strides, tap tables, program order, arena reuse — can be validated on a GPU-less machine against the
 oracle.  It never runs in the product path and says nothing about the CUDA kernels (tests/test_kernels_gpu.py
-does that on the B200).
+does that on the H100).
 """
 from __future__ import annotations
 

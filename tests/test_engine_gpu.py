@@ -180,7 +180,7 @@ def _tiny_model():
 
 
 def test_ddim_sampler_fused_path_matches_reference_golden():
-    """DDIMSampler.sample() (reference API) on the fused B200 path vs the reference's own 4-step sample."""
+    """DDIMSampler.sample() (reference API) on the fused H100 path vs the reference's own 4-step sample."""
     from oracle import ddim_oracle, unet_oracle
     from tooncrafter_b200 import layout
     from tooncrafter_b200.sampler import DDIMSampler
@@ -251,7 +251,7 @@ def test_general_sampler_path_and_decode_first_stage():
 
 
 def test_multicond_sampler_fused_path_matches_reference_golden():
-    """DDIMSampler_multicond (ddim_multiplecond.py:214-234) on the fused B200 path — the three guidance branches as ONE
+    """DDIMSampler_multicond (ddim_multiplecond.py:214-234) on the fused H100 path — the three guidance branches as ONE
     B = 3 UNet program per step + tc_ddim_step3 — vs the reference's own 4-step sample (golden) with the autocast oracle
     as yardstick, and vs the general three-pass path on the same GPU."""
     from make_golden_multicond import CFG_IMG, multicond_inputs

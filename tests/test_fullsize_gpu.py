@@ -1,4 +1,4 @@
-"""Parity of the programs bench.py actually times — BASELINE configs #2 / #4 geometry (inference_512_v1.0 UNet and
+"""Parity of the programs bench.py actually times — the clip and decode-only geometry (inference_512_v1.0 UNet and
 VAE at full width, T = 16 / 14, latent 40 x 64) — against (a) strided-subsample goldens produced by the UNMODIFIED
 reference at full size (tests/golden/make_golden_full.py, CPU fp32) and (b) the fp32 oracle on the GPU.
 

@@ -1,4 +1,4 @@
-"""Latency mode (SURVEY 8f-4): two GPUs share one clip, each evaluates one classifier-free-guidance branch per DDIM step
+"""Latency mode: two GPUs share one clip, each evaluates one classifier-free-guidance branch per DDIM step
 and the predictions are all-gathered.  The result must equal the single-GPU fused path (same algorithm, B = 1 + B = 1
 instead of one B = 2 forward).  The NCCL variant needs 2 GPUs (skipped on a single-GPU box, run with `gpurun --gpus 2`);
 the single-GPU variant runs the SAME two-rank protocol with both ranks time-sharing cuda:0 over gloo (collectives staged

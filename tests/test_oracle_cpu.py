@@ -1,6 +1,6 @@
 """CPU tests (no GPU): the oracle (oracle/*.py, our restatement of the reference algorithm) against
   (1) the committed golden outputs of the UNMODIFIED reference (tests/golden/, made by make_golden.py), and
-  (2) the reference itself when /root/reference is present (authoring container only),
+  (2) stored outputs of the unmodified reference UNet at another seed (tests/golden/live_reference_unet.npz),
 plus host-side logic: schedule known answers, state-dict key compatibility, C-ABI symbol export.
 """
 import json
@@ -62,7 +62,7 @@ def test_schedule_known_answers():
     assert abs(float(sched["scale_arr"][999]) - 0.7) < 1e-7 and abs(float(sched["scale_arr"][19]) - 0.985714) < 1e-6
     for k in ("betas", "alphas_cumprod", "sqrt_alphas_cumprod", "sqrt_one_minus_alphas_cumprod", "scale_arr"):
         assert np.array_equal(sched[k].numpy(), GOLD["sched_" + k]), k
-    # first step: direction coefficient sqrt(1 - a_prev - sigma^2) in fp32 (SURVEY App. C.11)
+    # first step: direction coefficient sqrt(1 - a_prev - sigma^2) in fp32
     co = ddim_oracle.step_coefficients(sched, tab, 49)
     assert co["sqrt_ac"] == 0.0 and co["sqrt_1mac"] == 1.0
     assert abs(co["dir_coef"] - 5.96e-8 ** 0.5) < 1e-6
@@ -134,41 +134,35 @@ def test_c_abi_library_exports_every_declared_symbol():
     assert lib.tc_version() >= 100
 
 
-@pytest.mark.skipif(not Path("/root/reference/lvdm").exists(), reason="reference tree only exists in the authoring container")
 def test_oracle_matches_live_reference_unet():
-    """Direct check against the imported, unmodified reference (different seed than the goldens)."""
-    import subprocess
-    code = (
-        "import sys, torch; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
-        "from oracle import ref_shims, unet_oracle\n"
-        "from tiny_config import *\n"
-        "from tooncrafter_b200 import synthetic, layout\n"
-        "ref = ref_shims.build_reference_unet(TINY_UNET).eval()\n"
-        "synthetic.fill_module_(ref, seed=5, prefix='model.diffusion_model.')\n"
-        "sd = {'model.diffusion_model.' + k: v for k, v in ref.state_dict().items()}\n"
-        "g = torch.Generator().manual_seed(3)\n"
-        "x = torch.randn(1, 8, TINY_T, 16, 16, generator=g); t = torch.tensor([250]);\n"
-        "ctx = torch.randn(1, 77 + 16 * TINY_T, TINY_CONTEXT_DIM, generator=g); fs = torch.tensor([7])\n"
-        "with torch.no_grad():\n"
-        "    a = ref(x, t, context=ctx, fs=fs)\n"
-        "    b = unet_oracle.unet_forward(sd, layout.unet_layout(TINY_UNET), x, t, ctx, fs, 'model.diffusion_model.')\n"
-        "err = (a - b).abs().max().item(); print('ERR', err); assert err < 2e-5\n"
-    ) % (str(HERE.parent), str(HERE))
-    # separate process: the reference's `lvdm` package must not shadow our own alias package in this one
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
+    """Against the unmodified original UNetModel (different seed than the goldens above): its output on the tiny
+    configuration is stored in tests/golden/live_reference_unet.npz (tests/golden/make_golden_live_reference.py); the
+    same seeded weights, filled by parameter name into this repository's UNetModel, feed the oracle."""
+    from tiny_config import TINY_CONTEXT_DIM, TINY_T, TINY_UNET
+    from tooncrafter_b200 import layout, synthetic
+    m = modules.UNetModel(**TINY_UNET).eval()
+    synthetic.fill_module_(m, seed=5, prefix="model.diffusion_model.")
+    sd = {"model.diffusion_model." + k: v for k, v in m.state_dict().items()}
+    g = torch.Generator().manual_seed(3)
+    x = torch.randn(1, 8, TINY_T, 16, 16, generator=g)
+    t = torch.tensor([250])
+    ctx = torch.randn(1, 77 + 16 * TINY_T, TINY_CONTEXT_DIM, generator=g)
+    fs = torch.tensor([7])
+    a = torch.from_numpy(np.load(HERE / "golden" / "live_reference_unet.npz")["out"])
+    with torch.no_grad():
+        b = unet_oracle.unet_forward(sd, layout.unet_layout(TINY_UNET), x, t, ctx, fs, "model.diffusion_model.")
+    err = (a - b).abs().max().item()
+    print("ERR", err)
+    assert err < 2e-5
 
 
 def test_reference_yaml_config_builds_our_classes_with_checkpoint_keys():
     """The reference's own configs/inference_512_v1.0.yaml, fed to OUR instantiate_from_config with this repository
     first on the import path (INTEGRATION.md 1): every hot-path `target:` resolves to our classes, their constructors
     accept the YAML's kwargs, and the resulting state dict carries the public checkpoint's keys.  Only the two OpenCLIP
-    towers (out of scope, need network weights) are swapped for Identity.  Needs /root/reference (authoring container)."""
-    import yaml
-    cfg_path = Path("/root/reference/configs/inference_512_v1.0.yaml")
-    if not cfg_path.exists():
-        pytest.skip("reference tree not present")
-    cfg = yaml.safe_load(cfg_path.read_text())["model"]
+    towers (out of scope, need network weights) are swapped for Identity.  The YAML's `model` section is stored parsed
+    in tests/golden/reference_model_config_512.json (tests/golden/make_golden_live_reference.py)."""
+    cfg = json.loads((HERE / "golden" / "reference_model_config_512.json").read_text())
     for k in ("cond_stage_config", "img_cond_stage_config"):
         cfg["params"][k] = {"target": "torch.nn.Identity"}
     cfg["params"]["unet_config"]["params"]["use_checkpoint"] = False            # inference.py:286
@@ -222,10 +216,9 @@ def test_utils_alias_covers_the_reference_surface():
     public function of the reference file (lvdm/modules/encoders/condition.py imports count_params from it)."""
     import ast
     import importlib
-    ref = Path("/root/reference/utils/utils.py")
-    names = ({n.name for n in ast.parse(ref.read_text()).body if isinstance(n, ast.FunctionDef)} if ref.exists() else
-             {"count_params", "check_istarget", "instantiate_from_config", "get_obj_from_str", "load_npz_from_dir",
-              "load_npz_from_paths", "resize_numpy_image", "setup_dist"})
+    # the public functions of the original utils/utils.py
+    names = {"count_params", "check_istarget", "instantiate_from_config", "get_obj_from_str", "load_npz_from_dir",
+             "load_npz_from_paths", "resize_numpy_image", "setup_dist"}
     sys.modules.pop("utils.utils", None)
     sys.modules.pop("utils", None)
     mod = importlib.import_module("utils.utils")

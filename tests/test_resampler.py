@@ -1,5 +1,5 @@
-"""Image-conditioning Resampler (SURVEY 8f-2): oracle pinned to the reference golden, state-dict keys pinned to the
-reference manifest, engine program checked on the CPU emulator and (gpu) on the B200 kernels."""
+"""Image-conditioning Resampler: oracle pinned to the reference golden, state-dict keys pinned to the
+reference manifest, engine program checked on the CPU emulator and (gpu) on the H100 kernels."""
 import json
 import sys
 from pathlib import Path

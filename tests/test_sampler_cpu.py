@@ -130,7 +130,7 @@ def test_fused_path_on_the_emulator_matches_reference_golden():
 
 
 def test_fused_multicond_path_on_the_emulator_matches_reference_golden():
-    """DDIMSampler_multicond (SURVEY 8f-3) on the fused path — one B = 3 UNet program per step + tc_ddim_step3 — with the
+    """DDIMSampler_multicond on the fused path — one B = 3 UNet program per step + tc_ddim_step3 — with the
     recorded programs interpreted on CPU, against the reference's own 4-step three-way-guidance sample
     (tests/golden/make_golden_multicond.py), and against the general (three-pass) path."""
     import numpy as np

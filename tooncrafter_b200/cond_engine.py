@@ -1,4 +1,4 @@
-"""ResamplerEngine: the image-conditioning Resampler (SURVEY 8f-2, "next" row) as a recorded program of C-ABI launches.
+"""ResamplerEngine: the image-conditioning Resampler as a recorded program of C-ABI launches.
 
 Reference: lvdm/modules/encoders/resampler.py:96-145 (Resampler.forward), :49-93 (PerceiverAttention: LayerNorm of the
 image tokens and of the latents, q from the latents, k/v from their concatenation, ONE softmax over all keys, scale

@@ -1,10 +1,11 @@
 // tooncrafter_b200 — attention kernels.
 //
-//  tc_attention           fused softmax(QK^T)V, head dim 64, tcgen05 MMAs (S = QK^T and O = PV) with TMEM
-//                         accumulators, TMA-staged Q/K/V tiles, fp32 online softmax, one query row per thread;
-//                         two query tiles per CTA ping-pong so one tile's softmax overlaps the other's MMAs.
+//  tc_attention           fused softmax(QK^T)V, head dim 64, one or two key/value segments (each with its own softmax,
+//                         outputs summed), mma.sync m16n8k16 with fp32 accumulators and an fp32 online softmax.
+//  tc_attention_wide      the same kernel for one head of up to 512 channels (VAE mid-block attention): scores stay
+//                         on chip; each CTA produces 256, 128 or 64 of the value channels (the widest that divides D).
 //  tc_temporal_attention  16-frame temporal self-attention, one (pixel, head) per warp, mma.sync 16x8x16 (HBM-bound).
-//  tc_softmax_rows        row softmax for the unfused d=512 VAE mid-block attention.
+//  tc_softmax_rows        row softmax over a stored score matrix.
 //
 // Reference sites: lvdm/modules/attention.py:81-209,365-412; lvdm/models/autoencoder_dualref.py:172-200,270-341.
 #include <stdlib.h>
@@ -13,28 +14,6 @@
 
 namespace {
 
-// ===================================================================================== fused attention (d = 64)
-constexpr int kQTile = 128;
-constexpr int kKVTile = 128;
-constexpr int kTileBytes = 128 * 64 * 2;  // 16 KiB: [128 rows][64 halfs], 128B-swizzled
-
-struct alignas(64) AttnKParams {
-    CUtensorMap tmQ;
-    CUtensorMap tmK[2];
-    CUtensorMap tmV[2];
-    int Lq, heads, n_seg;
-    int Lk[2];
-    int kv_div[2];
-    __half* out;
-    long long ldo;
-    float scale_log2;
-};
-
-__device__ __forceinline__ float fast_exp2(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
 __device__ __forceinline__ uint32_t pack_h2(float x, float y) {
     __half2 h = __floats2half2_rn(x, y);
     return *reinterpret_cast<uint32_t*>(&h);
@@ -46,328 +25,225 @@ __device__ __forceinline__ void split_h2(float x, float y, uint32_t& hi, uint32_
     hi = *reinterpret_cast<const uint32_t*>(&h);
     lo = pack_h2(x - f.x, y - f.y);
 }
+__device__ __forceinline__ void mma_m16n8k16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
+}
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+// 16-byte global -> shared copy, zero-filled when !ok
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, bool ok) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int kN>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(kN) : "memory"); }
 
-// Ping-pong over TWO query tiles per CTA with specialised warps:
-//   warps 0-3 / 4-7 : softmax warpgroups for query tile 0 / 1 (one query row per thread)
-//   warp 8          : MMA issuer   (S_w = Q_w K^T, O_w = P_w V; tcgen05, accumulators in TMEM)
-//   warp 9          : TMA producer (Q tiles once, K / V tiles double-buffered)
-// While one warpgroup runs its softmax (MUFU/ALU bound) the tensor core works on the other tile's MMAs.
-constexpr int kAttnThreads = 320;
-constexpr int kAttnTmemCols = 512;  // S0 [0,128) S1 [128,256) O0 [256,320) O1 [320,384)
+// ===================================================================================== fused attention
+// Flash-style: a CTA of 4 warps takes 64 query rows (16 per warp) of one (batch, head, value chunk); key tiles of 64
+// rows are staged in shared memory (K and V loads in separate cp.async groups, so S = Q K^T runs while V arrives).
+// Rows of D halfs are stored with their 16-byte chunks XOR-swizzled by (row & 7) so ldmatrix rows hit distinct banks.
+constexpr int kFaRows = 64;
+constexpr int kFaKeys = 64;
+constexpr int kFaThreads = 128;
 
-template <bool kTwoSeg>
-__global__ void __launch_bounds__(kAttnThreads, 1) tc_attn_kernel(const __grid_constant__ AttnKParams p) {
-    tc::pdl_launch_dependents();
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint8_t* sQ = smem;                     // 2 tiles
-    uint8_t* sK = smem + 2 * kTileBytes;    // 2 stages
-    uint8_t* sV = smem + 4 * kTileBytes;    // 2 stages
-    uint8_t* sP = smem + 6 * kTileBytes;    // 2 tiles x 2 sub-tiles
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 10 * kTileBytes);
-    uint64_t* bar_q = bars + 0;
-    uint64_t* k_full = bars + 1;    // [2]
-    uint64_t* k_free = bars + 3;    // [2]
-    uint64_t* v_full = bars + 5;    // [2]
-    uint64_t* v_free = bars + 7;    // [2]
-    uint64_t* s_full = bars + 9;    // [2] per query tile
-    uint64_t* o_full = bars + 11;   // [2]
-    uint64_t* p_ready = bars + 13;  // [2], 128 arrivals
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 15);
+struct FaSeg {
+    const __half* k;
+    const __half* v;
+    long long ldk, ldv;
+    int Lk, kv_div;        // K/V batch = query batch / kv_div
+};
+struct FaParams {
+    const __half* q;
+    long long ldq;
+    int Lq, heads;
+    int D;                 // q / k width per head
+    int DV, nv;            // value columns per CTA, value chunks per head (D = DV * nv)
+    int n_seg;
+    FaSeg seg[2];
+    __half* out;
+    long long ldo;
+    float scale_log2;
+    int split_p;
+};
 
-    const int tid = threadIdx.x;
-    const int warp = tid >> 5;
-    const int q0 = blockIdx.x * 2 * kQTile;
-    const int head = blockIdx.y;
-    const int qb = blockIdx.z;
-    const int ntiles = (q0 + kQTile < p.Lq) ? 2 : 1;
+// byte offset of 16-byte chunk c of row r in a swizzled tile with `cpr` chunks per row
+__device__ __forceinline__ uint32_t swz(int r, int c, int cpr) { return (uint32_t)((r * cpr + (c ^ (r & 7))) << 4); }
 
-    if (tid == 0) {
-        tc::mbar_init(bar_q, 1);
-        for (int i = 0; i < 2; ++i) {
-            tc::mbar_init(&k_full[i], 1);
-            tc::mbar_init(&k_free[i], 1);
-            tc::mbar_init(&v_full[i], 1);
-            tc::mbar_init(&v_free[i], 1);
-            tc::mbar_init(&s_full[i], 1);
-            tc::mbar_init(&o_full[i], 1);
-            tc::mbar_init(&p_ready[i], 128);
-        }
-        tc::fence_mbar_init();
+// kTwoSeg: up to two key/value segments, each with its own softmax, outputs summed (a second accumulator set)
+template <int kDV, bool kTwoSeg>
+__global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p) {
+    tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
+    extern __shared__ __align__(128) uint8_t fa_smem[];
+    const int D = p.D, cq = D / 8;                 // 16-byte chunks per q / k row
+    constexpr int cv = kDV / 8;                    // 16-byte chunks per v row
+    const uint32_t sQ = tc::smem_u32(fa_smem);
+    const uint32_t sK = sQ + (uint32_t)(kFaRows * D * 2);
+    const uint32_t sV = sK + (uint32_t)(kFaKeys * D * 2);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int q0 = blockIdx.x * kFaRows;
+    const int head = blockIdx.y / p.nv, vchunk = blockIdx.y - head * p.nv;
+    const int b = blockIdx.z;
+    const int qk_col = head * D, v_col = head * D + vchunk * kDV;
+
+    // ---- Q tile
+    for (int i = tid; i < kFaRows * cq; i += kFaThreads) {
+        const int r = i / cq, c = i - r * cq;
+        const bool ok = q0 + r < p.Lq;
+        const __half* src = p.q + ((long long)b * p.Lq + (ok ? q0 + r : 0)) * p.ldq + qk_col + c * 8;
+        cp_async16(sQ + swz(r, c, cq), src, ok);
     }
-    if (warp == 8) {
-        tc::tmem_alloc(tmem_ptr_smem, kAttnTmemCols);
-        tc::tmem_relinquish();
-    }
-    tc::tc_fence_before();
-    __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    tc::pdl_wait();   // prologue (barriers, TMEM) overlapped the predecessor; Q/K/V are its results
+    cp_async_commit();
 
-    if (warp == 9) {
-        // ------------------------------------------------------------------------------ TMA producer
-        // whole warp converged, one elected lane issues (see tc_gemm.cu for why `if (lane == 0)` is slow)
-        if (tc::elect_one()) {
-            tc::tma_prefetch_desc(&p.tmQ);
-            tc::mbar_arrive_expect_tx(bar_q, (uint32_t)(ntiles * kTileBytes));
-            for (int w = 0; w < ntiles; ++w) tc::tma_load_3d(sQ + w * kTileBytes, &p.tmQ, bar_q, head * 64, q0 + w * kQTile, qb);
-        }
-        __syncwarp();
-        int g = 0;
-        for (int seg = 0; seg < p.n_seg; ++seg) {
-            const int nblk = (p.Lk[seg] + kKVTile - 1) / kKVTile;
-            const int kvb = qb / p.kv_div[seg];
-            for (int j = 0; j < nblk; ++j, ++g) {
-                const int st = g & 1;
-                const uint32_t ph = (uint32_t)((g >> 1) & 1);
-                tc::mbar_wait(&k_free[st], ph ^ 1u);
-                if (tc::elect_one()) {
-                    tc::mbar_arrive_expect_tx(&k_full[st], kTileBytes);
-                    tc::tma_load_3d(sK + st * kTileBytes, &p.tmK[seg], &k_full[st], head * 64, j * kKVTile, kvb);
-                }
-                __syncwarp();
-                tc::mbar_wait(&v_free[st], ph ^ 1u);
-                if (tc::elect_one()) {
-                    tc::mbar_arrive_expect_tx(&v_full[st], kTileBytes);
-                    tc::tma_load_3d(sV + st * kTileBytes, &p.tmV[seg], &v_full[st], head * 64, j * kKVTile, kvb);
-                }
-                __syncwarp();
-            }
-        }
-    } else if (warp == 8) {
-        // ------------------------------------------------------------------------------ MMA issuer
-        {
-            const uint32_t sQ_a = tc::smem_u32(sQ), sK_a = tc::smem_u32(sK), sV_a = tc::smem_u32(sV), sP_a = tc::smem_u32(sP);
-            int G = 0;
-            for (int seg = 0; seg < p.n_seg; ++seg) G += (p.Lk[seg] + kKVTile - 1) / kKVTile;
-            // per-block key counts, walked in lock-step with the other roles
-            auto block_nk = [&](int gi) {
-                int seg = 0, j = gi;
-                while (true) {
-                    const int nb = (p.Lk[seg] + kKVTile - 1) / kKVTile;
-                    if (j < nb) break;
-                    j -= nb;
-                    ++seg;
-                }
-                const int left = p.Lk[seg] - j * kKVTile;
-                return left < kKVTile ? ((left + 15) & ~15) : kKVTile;
-            };
-            // S_w = Q_w K^T for key block in stage `st` (+ the commits that follow it); called by ONE elected lane
-            auto issue_s = [&](int w, int st, int nk, bool last_tile) {
-                const uint32_t idesc = tc::umma_idesc_f16(128, (uint32_t)nk, 0, 0);
-                const uint64_t qd = tc::umma_desc_sw128(sQ_a + (uint32_t)w * kTileBytes);
-                const uint64_t kd = tc::umma_desc_sw128(sK_a + (uint32_t)st * kTileBytes);
+    float ot[kTwoSeg ? kDV / 8 : 1][4];   // sum over the segments (two-segment form only)
 #pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    tc::umma_f16(tmem_base + (uint32_t)w * 128, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc, k != 0);
-                tc::umma_commit(&s_full[w]);
-                if (last_tile) tc::umma_commit(&k_free[st]);
-            };
-            tc::mbar_wait(bar_q, 0);
-            tc::mbar_wait(&k_full[0], 0);
-            tc::tc_fence_after();
-            {
-                const int nk = block_nk(0);
-                if (tc::elect_one()) {
-                    for (int w = 0; w < ntiles; ++w) issue_s(w, 0, nk, w == ntiles - 1);
-                }
-                __syncwarp();
+    for (int j = 0; j < (kTwoSeg ? kDV / 8 : 1); ++j) ot[j][0] = ot[j][1] = ot[j][2] = ot[j][3] = 0.f;
+    float o[kDV / 8][4];
+    const int g = lane >> 2, t4 = lane & 3;
+
+    for (int s = 0; s < (kTwoSeg ? p.n_seg : 1); ++s) {
+        const FaSeg sg = p.seg[s];
+        const long long kvb = b / sg.kv_div;
+#pragma unroll
+        for (int j = 0; j < kDV / 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+        float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+        for (int k0 = 0; k0 < sg.Lk; k0 += kFaKeys) {
+            __syncthreads();   // every warp is done with the previous K / V tile
+            for (int i = tid; i < kFaKeys * cq; i += kFaThreads) {
+                const int r = i / cq, c = i - r * cq;
+                const bool ok = k0 + r < sg.Lk;
+                cp_async16(sK + swz(r, c, cq), sg.k + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldk + qk_col + c * 8, ok);
             }
-            for (int g = 0; g < G; ++g) {
-                const int st = g & 1;
-                const int nk = block_nk(g);
-                const int nk_next = (g + 1 < G) ? block_nk(g + 1) : 0;
-                for (int w = 0; w < ntiles; ++w) {
-                    tc::mbar_wait(&p_ready[w], (uint32_t)(g & 1));
-                    if (w == 0) tc::mbar_wait(&v_full[st], (uint32_t)((g >> 1) & 1));
-                    if (g + 1 < G && w == 0) tc::mbar_wait(&k_full[(g + 1) & 1], (uint32_t)(((g + 1) >> 1) & 1));
-                    tc::tc_fence_after();
-                    if (tc::elect_one()) {
-                        const uint32_t idesc_o = tc::umma_idesc_f16(128, 64, 0, 1);  // B (= V tile) MN-major
-                        const uint64_t vd = tc::umma_desc_sw128(sV_a + (uint32_t)st * kTileBytes);
-                        for (int t = 0; t < nk / 16; ++t) {
-                            const uint64_t pd = tc::umma_desc_sw128(sP_a + (uint32_t)(2 * w + (t >> 2)) * kTileBytes) + (uint64_t)((t & 3) * 2);
-                            tc::umma_f16(tmem_base + 256 + (uint32_t)w * 64, pd, vd + (uint64_t)(t * 128), idesc_o, t != 0);
-                        }
-                        tc::umma_commit(&o_full[w]);
-                        if (w == ntiles - 1) tc::umma_commit(&v_free[st]);
-                        if (g + 1 < G) issue_s(w, (g + 1) & 1, nk_next, w == ntiles - 1);
-                    }
-                    __syncwarp();
+            cp_async_commit();
+            for (int i = tid; i < kFaKeys * cv; i += kFaThreads) {
+                const int r = i / cv, c = i - r * cv;
+                const bool ok = k0 + r < sg.Lk;
+                cp_async16(sV + swz(r, c, cv), sg.v + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldv + v_col + c * 8, ok);
+            }
+            cp_async_commit();
+            cp_async_wait<1>();   // Q and K have landed
+            __syncthreads();
+
+            // ---- S = Q K^T for this warp's 16 rows x 64 keys
+            float sc[8][4];
+#pragma unroll
+            for (int j = 0; j < 8; ++j) sc[j][0] = sc[j][1] = sc[j][2] = sc[j][3] = 0.f;
+            for (int kk = 0; kk < D / 16; ++kk) {
+                uint32_t a[4];
+                ldsm_x4(sQ + swz(warp * 16 + (lane & 15), 2 * kk + (lane >> 4), cq), a[0], a[1], a[2], a[3]);
+#pragma unroll
+                for (int np = 0; np < 4; ++np) {
+                    uint32_t b0, b1, b2, b3;
+                    ldsm_x4(sK + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), 2 * kk + ((lane >> 3) & 1), cq), b0, b1, b2, b3);
+                    mma_m16n8k16(sc[2 * np], a, b0, b1);
+                    mma_m16n8k16(sc[2 * np + 1], a, b2, b3);
                 }
             }
-        }
-    } else if ((warp >> 2) < ntiles) {
-        // ------------------------------------------------------------------------------ softmax warpgroups
-        const int w = warp >> 2;
-        const int row = tid & 127;
-        const uint32_t lane_off = ((uint32_t)((warp & 3) * 32)) << 16;
-        const uint32_t tmem_s = tmem_base + (uint32_t)w * 128 + lane_off;
-        const uint32_t tmem_o = tmem_base + 256 + (uint32_t)w * 64 + lane_off;
-        uint8_t* sPw = sP + (size_t)(2 * w) * kTileBytes;
-        float o_total[kTwoSeg ? 64 : 1];   // sum over segments (text + image cross attention) only when needed
-        if constexpr (kTwoSeg) {
+            // ---- online softmax (rows g and g + 8 of the warp; a row lives in the 4 lanes of a quad)
+            float mx0 = m0, mx1 = m1;
 #pragma unroll
-            for (int i = 0; i < 64; ++i) o_total[i] = 0.f;
-        }
-        float o_acc[64];
-        int g = 0;
-        for (int seg = 0; seg < p.n_seg; ++seg) {
-            const int Lk = p.Lk[seg];
-            const int nblk = (Lk + kKVTile - 1) / kKVTile;
-            float m_run = -INFINITY, l_run = 0.f;
+            for (int j = 0; j < 8; ++j) {
 #pragma unroll
-            for (int i = 0; i < 64; ++i) o_acc[i] = 0.f;
-            for (int j = 0; j < nblk; ++j, ++g) {
-                const int kv_left = Lk - j * kKVTile;
-                const int nvalid = kv_left < kKVTile ? kv_left : kKVTile;
-                const int nk = (nvalid + 15) & ~15;
-                tc::mbar_wait(&s_full[w], (uint32_t)(g & 1));
-                tc::tc_fence_after();
-                // ---- pass 1: row max.  Full blocks take the unpredicated path with 4 independent max chains
-                // (the serial FMNMX / FADD chains were the softmax warps' critical path: 2 warps per scheduler).
-                float m_blk;
-                const bool full = (nvalid == kKVTile);
-                if (full) {
-                    float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        uint32_t r[32];
-                        tc::tmem_ld32(tmem_s + (uint32_t)(c * 32), r);
-                        tc::tmem_ld_wait();
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4) {
-                            mx[0] = fmaxf(mx[0], __uint_as_float(r[i]));
-                            mx[1] = fmaxf(mx[1], __uint_as_float(r[i + 1]));
-                            mx[2] = fmaxf(mx[2], __uint_as_float(r[i + 2]));
-                            mx[3] = fmaxf(mx[3], __uint_as_float(r[i + 3]));
-                        }
-                    }
-                    m_blk = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-                } else {
-                    m_blk = -INFINITY;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        if (c * 16 < nk) {
-                            uint32_t r[16];
-                            tc::tmem_ld16(tmem_s + (uint32_t)(c * 16), r);
-                            tc::tmem_ld_wait();
-#pragma unroll
-                            for (int i = 0; i < 16; ++i)
-                                if (c * 16 + i < nvalid) m_blk = fmaxf(m_blk, __uint_as_float(r[i]));
-                        }
-                    }
-                }
-                const float m_new = fmaxf(m_run, m_blk);
-                const float m_scaled = m_new * p.scale_log2;
-                const float alpha = fast_exp2(m_run * p.scale_log2 - m_scaled);
-                // ---- pass 2: p = exp2(s * scale - m * scale), row sum, P tile (fp16, K-major, 128B swizzle) to smem
-                float l_blk;
-                if (full) {
-                    float ls[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        uint32_t r[32];
-                        tc::tmem_ld32(tmem_s + (uint32_t)(c * 32), r);
-                        tc::tmem_ld_wait();
-                        uint32_t pk[16];
-#pragma unroll
-                        for (int i = 0; i < 32; i += 4) {
-                            const float e0 = fast_exp2(fmaf(__uint_as_float(r[i]), p.scale_log2, -m_scaled));
-                            const float e1 = fast_exp2(fmaf(__uint_as_float(r[i + 1]), p.scale_log2, -m_scaled));
-                            const float e2 = fast_exp2(fmaf(__uint_as_float(r[i + 2]), p.scale_log2, -m_scaled));
-                            const float e3 = fast_exp2(fmaf(__uint_as_float(r[i + 3]), p.scale_log2, -m_scaled));
-                            ls[0] += e0;
-                            ls[1] += e1;
-                            ls[2] += e2;
-                            ls[3] += e3;
-                            pk[i / 2] = pack_h2(e0, e1);
-                            pk[i / 2 + 1] = pack_h2(e2, e3);
-                        }
-                        uint8_t* sub = sPw + (c >> 1) * kTileBytes + row * 128;
-                        const int ch0 = (c & 1) * 4;
-#pragma unroll
-                        for (int q4 = 0; q4 < 4; ++q4)
-                            *reinterpret_cast<uint4*>(sub + (((ch0 + q4) ^ (row & 7)) << 4)) =
-                                make_uint4(pk[4 * q4], pk[4 * q4 + 1], pk[4 * q4 + 2], pk[4 * q4 + 3]);
-                    }
-                    l_blk = (ls[0] + ls[1]) + (ls[2] + ls[3]);
-                } else {
-                    l_blk = 0.f;
-#pragma unroll
-                    for (int c = 0; c < 8; ++c) {
-                        if (c * 16 < nk) {
-                            uint32_t r[16];
-                            tc::tmem_ld16(tmem_s + (uint32_t)(c * 16), r);
-                            tc::tmem_ld_wait();
-                            uint32_t pk[8];
-#pragma unroll
-                            for (int i = 0; i < 16; i += 2) {
-                                float e0 = fast_exp2(fmaf(__uint_as_float(r[i]), p.scale_log2, -m_scaled));
-                                float e1 = fast_exp2(fmaf(__uint_as_float(r[i + 1]), p.scale_log2, -m_scaled));
-                                e0 = (c * 16 + i < nvalid) ? e0 : 0.f;
-                                e1 = (c * 16 + i + 1 < nvalid) ? e1 : 0.f;
-                                l_blk += e0 + e1;
-                                pk[i / 2] = pack_h2(e0, e1);
-                            }
-                            uint8_t* sub = sPw + (c >> 2) * kTileBytes + row * 128;
-                            const int ch0 = (c & 3) * 2;
-                            *reinterpret_cast<uint4*>(sub + (((ch0) ^ (row & 7)) << 4)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                            *reinterpret_cast<uint4*>(sub + (((ch0 + 1) ^ (row & 7)) << 4)) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                        }
-                    }
-                }
-                l_run = l_run * alpha + l_blk;
-                m_run = m_new;
-                tc::fence_proxy_async_smem();
-                tc::tc_fence_before();
-                tc::mbar_arrive(&p_ready[w]);
-                // O_blk of this block: o_acc = o_acc * alpha + P V
-                tc::mbar_wait(&o_full[w], (uint32_t)(g & 1));
-                tc::tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    uint32_t r[32];
-                    tc::tmem_ld32(tmem_o + (uint32_t)(c * 32), r);
-                    tc::tmem_ld_wait();
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o_acc[c * 32 + i] = fmaf(o_acc[c * 32 + i], alpha, __uint_as_float(r[i]));
+                for (int i = 0; i < 2; ++i) {
+                    const bool key_ok = k0 + 8 * j + 2 * t4 + i < sg.Lk;
+                    sc[j][i] = key_ok ? sc[j][i] * p.scale_log2 : -INFINITY;
+                    sc[j][2 + i] = key_ok ? sc[j][2 + i] * p.scale_log2 : -INFINITY;
+                    mx0 = fmaxf(mx0, sc[j][i]);
+                    mx1 = fmaxf(mx1, sc[j][2 + i]);
                 }
             }
-            const float inv_l = 1.0f / l_run;
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+            mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+            const float al0 = exp2f(m0 - mx0), al1 = exp2f(m1 - mx1);   // 0 on the first tile (m = -inf)
+            m0 = mx0;
+            m1 = mx1;
+            l0 *= al0;
+            l1 *= al1;
+#pragma unroll
+            for (int j = 0; j < kDV / 8; ++j) {
+                o[j][0] *= al0;
+                o[j][1] *= al0;
+                o[j][2] *= al1;
+                o[j][3] *= al1;
+            }
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                sc[j][0] = exp2f(sc[j][0] - m0);
+                sc[j][1] = exp2f(sc[j][1] - m0);
+                sc[j][2] = exp2f(sc[j][2] - m1);
+                sc[j][3] = exp2f(sc[j][3] - m1);
+                l0 += sc[j][0] + sc[j][1];
+                l1 += sc[j][2] + sc[j][3];
+            }
+            cp_async_wait<0>();   // V has landed
+            __syncthreads();
+            // ---- O += P V (P as the A operand straight from the score fragments)
+#pragma unroll
+            for (int kb = 0; kb < 4; ++kb) {
+                uint32_t pa[4], pl[4];
+                split_h2(sc[2 * kb][0], sc[2 * kb][1], pa[0], pl[0]);
+                split_h2(sc[2 * kb][2], sc[2 * kb][3], pa[1], pl[1]);
+                split_h2(sc[2 * kb + 1][0], sc[2 * kb + 1][1], pa[2], pl[2]);
+                split_h2(sc[2 * kb + 1][2], sc[2 * kb + 1][3], pa[3], pl[3]);
+                const int mrow = kb * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
+#pragma unroll
+                for (int nd = 0; nd < kDV / 8; nd += 2) {
+                    uint32_t b0, b1, b2, b3;
+                    ldsm_x4_t(sV + swz(mrow, nd + (lane >> 4), cv), b0, b1, b2, b3);
+                    if (p.split_p) {
+                        mma_m16n8k16(o[nd], pl, b0, b1);
+                        mma_m16n8k16(o[nd + 1], pl, b2, b3);
+                    }
+                    mma_m16n8k16(o[nd], pa, b0, b1);
+                    mma_m16n8k16(o[nd + 1], pa, b2, b3);
+                }
+            }
+        }
+        l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+        l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+        l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+        const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+#pragma unroll
+        for (int j = 0; j < kDV / 8; ++j) {
+            o[j][0] *= inv0;
+            o[j][1] *= inv0;
+            o[j][2] *= inv1;
+            o[j][3] *= inv1;
             if constexpr (kTwoSeg) {
-#pragma unroll
-                for (int i = 0; i < 64; ++i) o_total[i] += o_acc[i] * inv_l;
-            } else {
-#pragma unroll
-                for (int i = 0; i < 64; ++i) o_acc[i] *= inv_l;
-            }
-        }
-        const float* o_fin = kTwoSeg ? o_total : o_acc;
-        const int qrow = q0 + w * kQTile + row;
-        if (qrow < p.Lq) {
-            __half* dst = p.out + ((long long)qb * p.Lq + qrow) * p.ldo + head * 64;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                __half2 h[4];
-#pragma unroll
-                for (int i = 0; i < 4; ++i) h[i] = __floats2half2_rn(o_fin[c * 8 + 2 * i], o_fin[c * 8 + 2 * i + 1]);
-                uint4 u;
-                u.x = *reinterpret_cast<uint32_t*>(&h[0]);
-                u.y = *reinterpret_cast<uint32_t*>(&h[1]);
-                u.z = *reinterpret_cast<uint32_t*>(&h[2]);
-                u.w = *reinterpret_cast<uint32_t*>(&h[3]);
-                reinterpret_cast<uint4*>(dst)[c] = u;
+                ot[j][0] += o[j][0];
+                ot[j][1] += o[j][1];
+                ot[j][2] += o[j][2];
+                ot[j][3] += o[j][3];
             }
         }
     }
-
-    tc::tc_fence_before();
-    __syncthreads();
-    if (warp == 8) {
-        tc::tc_fence_after();
-        tc::tmem_dealloc(tmem_base, kAttnTmemCols);
+    if constexpr (kTwoSeg) {
+#pragma unroll
+        for (int j = 0; j < kDV / 8; ++j) {
+            o[j][0] = ot[j][0];
+            o[j][1] = ot[j][1];
+            o[j][2] = ot[j][2];
+            o[j][3] = ot[j][3];
+        }
+    }
+    const int r0 = q0 + warp * 16 + g, r1 = r0 + 8;
+    __half* o0p = p.out + ((long long)b * p.Lq + r0) * p.ldo + v_col + 2 * t4;
+    __half* o1p = p.out + ((long long)b * p.Lq + r1) * p.ldo + v_col + 2 * t4;
+#pragma unroll
+    for (int j = 0; j < kDV / 8; ++j) {
+        if (r0 < p.Lq) *reinterpret_cast<uint32_t*>(o0p + 8 * j) = pack_h2(o[j][0], o[j][1]);
+        if (r1 < p.Lq) *reinterpret_cast<uint32_t*>(o1p + 8 * j) = pack_h2(o[j][2], o[j][3]);
     }
 }
 
@@ -478,16 +354,10 @@ __global__ void temporal_attn_kernel(const __half* __restrict__ q, const __half*
 }
 
 // ===================================================================================== temporal attention, T <= 16
-// One warp per (batch, pixel, head): the whole problem is a 16 x 16 x 64 attention, far below the 128-row tcgen05 tile,
+// One warp per (batch, pixel, head): the whole problem is a 16 x 16 x 64 attention, far below a 64-row wgmma tile,
 // and the kernel is HBM-bound (reads q, k, v once, writes o once).  S = Q K^T and O = P V use warp-level
 // mma.sync.m16n8k16 with fragments loaded straight from global memory (Q, K) or via ldmatrix.trans from a
 // swizzled 2 KiB smem tile (V); softmax in fp32 on the accumulator fragments.
-__device__ __forceinline__ void mma_m16n8k16(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-        : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __global__ void __launch_bounds__(128) temporal_attn_mma_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
                                                                 const __half* __restrict__ v, long long ld,
                                                                 __half* __restrict__ out, long long ldo, int B, int T,
@@ -646,18 +516,39 @@ __global__ void softmax_rows_kernel(__half* __restrict__ s, long long lds, int r
 
 using namespace tc_host;
 
-int tc_attention_v3(const TcAttention* d, int poly_of_8, cudaStream_t stream);   // tc_attn3.cu
-int tc_attention_xs(const TcAttention* d, cudaStream_t stream);                    // tc_attn3.cu (small K/V, 1-2 segments)
-
-// TC_ATTN_IMPL=v2 keeps single-segment problems on the second-generation kernel below (A/B runs);
-// TC_ATTN_POLY=n (0..4) sets how many of every 8 exponential pairs the v3 kernel evaluates on the FMA pipe.
-static int attn_impl_v3() {
-    const char* e = getenv("TC_ATTN_IMPL");
-    return !(e && e[0] == 'v' && e[1] == '2');
+template <int kDV, bool kTwoSeg>
+static int launch_flash_kernel(const FaParams& p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
+    static bool attr_set = false;
+    if (!attr_set) {
+        int rc = check_cuda(cudaFuncSetAttribute(flash_attn_kernel<kDV, kTwoSeg>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 227 * 1024),
+                            "cudaFuncSetAttribute(flash_attn_kernel)");
+        if (rc) return rc;
+        attr_set = true;
+    }
+    tc_host::launch(flash_attn_kernel<kDV, kTwoSeg>, grid, dim3(kFaThreads), smem_bytes, stream, 1, p);
+    return TC_OK;
 }
-static int attn_poly() {
-    const char* e = getenv("TC_ATTN_POLY");
-    return (e && e[0] >= '0' && e[0] <= '4') ? e[0] - '0' : 0;
+
+// split_p: P as fp16 hi + lo parts for the PV product when few keys average its rounding (cross attention: 77 + 16 keys)
+static int launch_flash(const FaParams& p0, int batches, int Lk_max, cudaStream_t stream) {
+    FaParams p = p0;
+    p.split_p = Lk_max <= 512 ? 1 : 0;
+    const size_t smem_bytes = (size_t)(2 * kFaRows * p.D + kFaKeys * p.DV) * 2 + 128;
+    dim3 grid((p.Lq + kFaRows - 1) / kFaRows, p.heads * p.nv, batches);
+    int rc;
+    if (p.n_seg == 2)
+        rc = launch_flash_kernel<64, true>(p, grid, smem_bytes, stream);        // tc_attention only: DV = D = 64
+    else if (p.DV == 64)
+        rc = launch_flash_kernel<64, false>(p, grid, smem_bytes, stream);
+    else if (p.DV == 128)
+        rc = launch_flash_kernel<128, false>(p, grid, smem_bytes, stream);
+    else
+        rc = launch_flash_kernel<256, false>(p, grid, smem_bytes, stream);
+    if (rc) return rc;
+    count_launch();
+    TC_CHECK_LAUNCH("flash_attn_kernel");
+    return TC_OK;
 }
 
 extern "C" int tc_attention(const TcAttention* d, void* stream_v) {
@@ -666,73 +557,77 @@ extern "C" int tc_attention(const TcAttention* d, void* stream_v) {
     TC_CHECK_ARG(d->n_seg == 1 || d->n_seg == 2, "tc_attention: n_seg must be 1 or 2");
     TC_CHECK_ARG(d->q_batches > 0 && d->Lq > 0 && d->heads > 0, "tc_attention: empty problem");
     TC_CHECK_ARG(d->ldq % 8 == 0 && d->ldo % 8 == 0, "tc_attention: strides must be multiples of 8");
-    if (d->n_seg == 1 && attn_impl_v3()) {
-        TC_CHECK_ARG(d->k[0] && d->v[0] && d->Lk[0] > 0 && d->kv_div[0] > 0, "tc_attention: bad kv segment");
-        TC_CHECK_ARG(d->ldk[0] % 8 == 0 && d->ldv[0] % 8 == 0, "tc_attention: kv strides must be multiples of 8");
-        return tc_attention_v3(d, attn_poly(), stream);
-    }
-    if (attn_impl_v3()) {
-        // short K/V (the 77 text + 16 image tokens of the cross attentions): resident-K/V kernel when the shape fits
-        bool ok = true;
-        for (int s = 0; s < d->n_seg; ++s)
-            ok = ok && d->k[s] && d->v[s] && d->Lk[s] > 0 && d->kv_div[s] > 0 && d->ldk[s] % 8 == 0 && d->ldv[s] % 8 == 0;
-        if (ok) {
-            const int rc = tc_attention_xs(d, stream);
-            if (rc != TC_ERR_INVALID) return rc;
-        }
-    }
-    AttnKParams p;
+    TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->q) | reinterpret_cast<uintptr_t>(d->out)) & 15) == 0,
+                 "tc_attention: operands must be 16-byte aligned");
+    FaParams p;
     memset(&p, 0, sizeof(p));
-    const uint32_t box[3] = {64, 128, 1};
-    {
-        uint64_t dims[3] = {(uint64_t)d->heads * 64, (uint64_t)d->Lq, (uint64_t)d->q_batches};
-        uint64_t str[2] = {(uint64_t)d->ldq * 2, (uint64_t)d->Lq * (uint64_t)d->ldq * 2};
-        const CUtensorMap* m = get_tensor_map(d->q, 3, dims, str, box);
-        if (!m) return TC_ERR_CUDA;
-        p.tmQ = *m;
-    }
+    int Lk_max = 0;
     for (int s = 0; s < d->n_seg; ++s) {
         TC_CHECK_ARG(d->k[s] && d->v[s] && d->Lk[s] > 0 && d->kv_div[s] > 0, "tc_attention: bad kv segment");
         TC_CHECK_ARG(d->ldk[s] % 8 == 0 && d->ldv[s] % 8 == 0, "tc_attention: kv strides must be multiples of 8");
-        const int kvb = (d->q_batches + d->kv_div[s] - 1) / d->kv_div[s];
-        uint64_t dims[3] = {(uint64_t)d->heads * 64, (uint64_t)d->Lk[s], (uint64_t)kvb};
-        uint64_t strk[2] = {(uint64_t)d->ldk[s] * 2, (uint64_t)d->Lk[s] * (uint64_t)d->ldk[s] * 2};
-        uint64_t strv[2] = {(uint64_t)d->ldv[s] * 2, (uint64_t)d->Lk[s] * (uint64_t)d->ldv[s] * 2};
-        const CUtensorMap* mk = get_tensor_map(d->k[s], 3, dims, strk, box);
-        const CUtensorMap* mv = get_tensor_map(d->v[s], 3, dims, strv, box);
-        if (!mk || !mv) return TC_ERR_CUDA;
-        p.tmK[s] = *mk;
-        p.tmV[s] = *mv;
-        p.Lk[s] = d->Lk[s];
-        p.kv_div[s] = d->kv_div[s];
+        TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->k[s]) | reinterpret_cast<uintptr_t>(d->v[s])) & 15) == 0,
+                     "tc_attention: operands must be 16-byte aligned");
+        p.seg[s].k = reinterpret_cast<const __half*>(d->k[s]);
+        p.seg[s].v = reinterpret_cast<const __half*>(d->v[s]);
+        p.seg[s].ldk = d->ldk[s];
+        p.seg[s].ldv = d->ldv[s];
+        p.seg[s].Lk = d->Lk[s];
+        p.seg[s].kv_div = d->kv_div[s];
+        Lk_max = d->Lk[s] > Lk_max ? d->Lk[s] : Lk_max;
     }
+    p.q = reinterpret_cast<const __half*>(d->q);
+    p.ldq = d->ldq;
     p.Lq = d->Lq;
     p.heads = d->heads;
+    p.D = 64;
+    p.DV = 64;
+    p.nv = 1;
     p.n_seg = d->n_seg;
     p.out = reinterpret_cast<__half*>(d->out);
     p.ldo = d->ldo;
     p.scale_log2 = d->scale * 1.4426950408889634f;
-    const size_t smem_bytes = 10 * kTileBytes + 1024 + 256;
-    static bool attr2_set = false;
-    if (!attr2_set) {
-        int rc = check_cuda(cudaFuncSetAttribute(tc_attn_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 (int)smem_bytes),
-                            "cudaFuncSetAttribute(tc_attn_kernel<false>)");
-        if (rc) return rc;
-        rc = check_cuda(cudaFuncSetAttribute(tc_attn_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             (int)smem_bytes),
-                        "cudaFuncSetAttribute(tc_attn_kernel<true>)");
-        if (rc) return rc;
-        attr2_set = true;
-    }
-    dim3 grid((d->Lq + 2 * kQTile - 1) / (2 * kQTile), d->heads, d->q_batches);
-    if (d->n_seg == 2)
-        tc_host::launch(tc_attn_kernel<true>, dim3(grid), dim3(kAttnThreads), smem_bytes, stream, 1, p);
-    else
-        tc_host::launch(tc_attn_kernel<false>, dim3(grid), dim3(kAttnThreads), smem_bytes, stream, 1, p);
-    count_launch();
-    TC_CHECK_LAUNCH("tc_attn_kernel");
-    return TC_OK;
+    return launch_flash(p, d->q_batches, Lk_max, stream);
+}
+
+extern "C" int tc_attention_wide(const void* q, const void* k, const void* v, long long ldq, long long ldk, long long ldv,
+                                 void* out, long long ldo, int batches, int Lq, int Lk, int D, float scale, void* stream_v) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    TC_CHECK_ARG(q && k && v && out, "tc_attention_wide: null pointer");
+    TC_CHECK_ARG(batches > 0 && Lq > 0 && Lk > 0, "tc_attention_wide: empty problem");
+    TC_CHECK_ARG(D >= 64 && D <= 512 && D % 64 == 0 && (D <= 256 || D % 128 == 0),
+                 "tc_attention_wide: head dim must be a multiple of 64 (of 128 above 256), at most 512");
+    TC_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "tc_attention_wide: strides must be multiples of 8");
+    TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+                   reinterpret_cast<uintptr_t>(out)) & 15) == 0, "tc_attention_wide: operands must be 16-byte aligned");
+    FaParams p;
+    memset(&p, 0, sizeof(p));
+    p.q = reinterpret_cast<const __half*>(q);
+    p.ldq = ldq;
+    p.Lq = Lq;
+    p.heads = 1;
+    p.D = D;
+    // value columns per CTA: the widest chunk that divides D (each CTA recomputes Q K^T, so fewer chunks = fewer flops;
+    // D = 192 takes three 64-column chunks)
+    p.DV = D % 256 == 0 ? 256 : (D % 128 == 0 ? 128 : 64);
+    p.nv = D / p.DV;
+    TC_CHECK_ARG(p.nv * p.DV == D, "tc_attention_wide: value chunk does not divide the head dim");
+    p.n_seg = 1;
+    p.seg[0].k = reinterpret_cast<const __half*>(k);
+    p.seg[0].v = reinterpret_cast<const __half*>(v);
+    p.seg[0].ldk = ldk;
+    p.seg[0].ldv = ldv;
+    p.seg[0].Lk = Lk;
+    p.seg[0].kv_div = 1;
+    p.out = reinterpret_cast<__half*>(out);
+    p.ldo = ldo;
+    p.scale_log2 = scale * 1.4426950408889634f;
+    return launch_flash(p, batches, Lk, stream);
+}
+
+extern "C" int tc_debug_read_attn_trace(unsigned long long* host_dst, int count) {
+    (void)host_dst;
+    (void)count;
+    return fail(TC_ERR_INVALID, "tc_debug_read_attn_trace: the attention kernel records no timeline");
 }
 
 extern "C" int tc_temporal_attention(const void* q, const void* k, const void* v, long long ld, void* out,

@@ -1,8 +1,7 @@
-// tooncrafter_b200 — shared device-side primitives for the sm_100a kernels.
+// tooncrafter_b200 — shared device-side primitives for the sm_90a kernels.
 //
-// Thin inline-PTX wrappers around the Blackwell async machinery: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the UMMA shared-memory /
-// instruction descriptors.  Everything here is sm_100a-only.
+// Thin inline-PTX wrappers around the Hopper async machinery: mbarrier, TMA (cp.async.bulk.tensor),
+// wgmma (warpgroup MMA with shared-memory descriptors), clusters and programmatic dependent launch.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -107,62 +106,29 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const void* tmap, uint64_
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05: tensor memory + 5th-gen tensor core MMA
+// wgmma: warpgroup MMA (sm_90a), A and B from shared memory, fp32 accumulators in registers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kN>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kN) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem] * B[smem]   (kind::f16: fp16/bf16 operands, fp32 accumulate)
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                         uint32_t accumulate) {
+// D[64 x 32] += A[64 x 16] * B[16 x 32]: fp16 operands, both K-major in shared memory; this thread's 16 accumulators
+// (row = 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column = 8 * (i >> 2) + 2 * (lane % 4) + (i & 1))
+__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// all previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
+        "setp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(desc_a), "l"(desc_b));
 }
 
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns (thread i <- lane i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
 // ---- programmatic dependent launch: every kernel of this library is launched with the programmatic-stream-serialization
 // attribute (tc_host::launch), lets its successor's CTAs start early (launch_dependents) and must execute pdl_wait()
 // before its first access to global memory a predecessor may have written — and EVERY kernel must execute it, otherwise
@@ -188,47 +154,8 @@ template <int kN>
 __device__ __forceinline__ void bulk_wait_group() {
     asm volatile("cp.async.bulk.wait_group %0;" ::"n"(kN) : "memory");
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM: this warp's 32 lanes x N consecutive 32-bit columns (lane i <- thread i)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-        "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-        "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows = TMEM lanes, K-major, 16-bit elements packed two per
-// 32-bit column, K = 16 per instruction = 8 columns) is read from tensor memory
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-
 // ---------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) variants: two SMs of a cluster cooperate on one M = 256 tile
+// clusters
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
@@ -250,138 +177,20 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta)
         "r"(cta)
         : "memory");
 }
-// TMA loads issued by either CTA of a pair; completion bytes are credited to the LEADER CTA's mbarrier
-// (shared::cluster address of the barrier with the CTA-rank bit cleared)
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const void* tmap, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
-                                                 int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1),
-        "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* dst_smem, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_pair() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A[128 rows per CTA] * B[N/2 rows per CTA]   (M = 256 across the pair)
-__device__ __forceinline__ void umma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                              uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// completion of all prior pair-MMAs arrives on the mbarrier at this smem offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_pair(uint64_t* bar) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-            smem_u32(bar)),
-        "h"((uint16_t)3)
-        : "memory");
-}
-
 // ---------------------------------------------------------------------------------------------
-// UMMA descriptors
+// wgmma shared-memory matrix descriptor, 128-byte swizzle, K-major rows of 128 bytes packed densely (8-row swizzle
+// atoms of 1024 B, as TMA writes a box whose inner extent is 64 halfs with CU_TENSOR_MAP_SWIZZLE_128B).
+//   bits [0,14) start address >> 4     bits [16,30) leading byte offset >> 4 (unused for swizzled K-major)
+//   bits [32,46) stride byte offset >> 4 (1024 B between 8-row groups)     bits [62,64) layout (1 = SWIZZLE_128B)
+// Advancing K by 16 halfs inside the swizzle row adds 32 bytes (+2) to the start address field.
 // ---------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor, 128-byte swizzle, rows of 128 bytes packed densely
-// (8-row swizzle atoms of 1024 B).  Valid both for a K-major operand tile [rows][64 halfs]
-// (SBO = 1024 B between 8-row groups) and for an MN-major operand tile [k][64 halfs]
-// (SBO = 1024 B between 8-k groups; a single 64-wide MN chunk so LBO is unused).
-//   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version (1 on sm_100)
-//   bits [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-    d |= static_cast<uint64_t>(1) << 16;           // LBO (ignored for swizzled K-major; canonical value 1)
-    d |= static_cast<uint64_t>(1024 >> 4) << 32;   // SBO
-    d |= static_cast<uint64_t>(1) << 46;           // version
-    d |= static_cast<uint64_t>(2) << 61;           // SWIZZLE_128B
+    d |= static_cast<uint64_t>(1) << 16;
+    d |= static_cast<uint64_t>(1024 >> 4) << 32;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
-}
-
-// Instruction descriptor for kind::f16 with fp16 A/B, fp32 D.
-//   [4,6) c_format (1 = f32)  [7,10) a_format (0 = f16)  [10,13) b_format  [15] a_major  [16] b_major
-//   [17,23) N >> 3            [24,29) M >> 4
-__device__ __forceinline__ uint32_t umma_idesc_f16(uint32_t M, uint32_t N, uint32_t a_mn_major, uint32_t b_mn_major) {
-    uint32_t d = 0;
-    d |= 1u << 4;
-    d |= (a_mn_major & 1u) << 15;
-    d |= (b_mn_major & 1u) << 16;
-    d |= (N >> 3) << 17;
-    d |= (M >> 4) << 24;
-    return d;
-}
-
-// ---------------------------------------------------------------------------------------------
-// packed fp32 pairs (sm_100 FFMA2 / FADD2 / FMUL2): one issue slot per TWO values.  The pipe rate per value is the
-// scalar one (measured: profiles/r02_pipe_rates.txt), the win is instruction issue, which bounds the GEMM epilogues
-// and the attention softmax.
-// ---------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ f32x2 pk2u(uint32_t lo, uint32_t hi) {
-    f32x2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpk2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ void unpk2u(f32x2 v, uint32_t& lo, uint32_t& hi) { asm("mov.b64 {%0, %1}, %2;" : "=r"(lo), "=r"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ f32x2 add2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f32x2 sub2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) {
-    f32x2 r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-// fp16 pair from an fp32 pair (low element -> low half)
-__device__ __forceinline__ uint32_t h2_from_f2(f32x2 v) {
-    float lo, hi;
-    unpk2(v, lo, hi);
-    uint32_t r;
-    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-    return r;
-}
-// fp32 pair from an fp16 pair
-__device__ __forceinline__ f32x2 f2_from_h2(uint32_t h) {
-    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
-    return pk2(f.x, f.y);
 }
 
 __device__ __forceinline__ float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
@@ -407,7 +216,7 @@ __device__ __forceinline__ float erf_fast(float x) {
 }
 __device__ __forceinline__ float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erf_fast(x * 0.70710678118654752f)); }
 
-// a * GELU(x) for the GEGLU epilogue (which is instruction-issue bound: 38 thread instructions per output measured).
+// a * GELU(x): the cheap form of the GEGLU product.
 // GELU(x) = x * Phi(x) with Phi(x) = 1 - h for x >= 0 and h for x < 0, h = 0.5 * (1 + a1 z + ... + a6 z^6)^-16,
 // z = |x| / sqrt(2): the same A&S 7.1.28 polynomial with 2^(-i/2) (the x/sqrt(2)) and 2^(1/16) (the 0.5) folded into its
 // coefficients: 6 FFMA + 4 FMUL + 1 MUFU + FADD + FSEL + 2 FMUL, |GELU error| <= 8e-7.
@@ -429,32 +238,5 @@ __device__ __forceinline__ float geglu_mul(float a, float x) {
     return (a * x) * phi;
 }
 
-
-// Two GEGLU products at once: (a * x * Phi(x)) for the pairs a = (a0, a1), x = (g0, g1) — the same A&S 7.1.28 form as
-// geglu_mul with the polynomial, the four squarings and the final products on packed FFMA2 / FMUL2 (half the issue
-// slots), |x| by clearing sign bits (ALU pipe) and the reciprocal on MUFU.
-__device__ __forceinline__ f32x2 geglu_mul2(f32x2 a, f32x2 x) {
-    uint32_t x0, x1;
-    unpk2u(x, x0, x1);
-    const f32x2 ax = pk2u(x0 & 0x7fffffffu, x1 & 0x7fffffffu);
-    f32x2 t = fma2(ax, pk2(5.6212996640e-06f, 5.6212996640e-06f), pk2(5.1055209009e-05f, 5.1055209009e-05f));
-    t = fma2(t, ax, pk2(3.9686137011e-05f, 3.9686137011e-05f));
-    t = fma2(t, ax, pk2(3.4227392389e-03f, 3.4227392389e-03f));
-    t = fma2(t, ax, pk2(2.2076998457e-02f, 2.2076998457e-02f));
-    t = fma2(t, ax, pk2(5.2075163037e-02f, 5.2075163037e-02f));
-    t = fma2(t, ax, pk2(1.0442737824e+00f, 1.0442737824e+00f));
-    t = mul2(t, t);
-    t = mul2(t, t);
-    t = mul2(t, t);
-    t = mul2(t, t);
-    float t0, t1, h0, h1;
-    unpk2(t, t0, t1);
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(h0) : "f"(t0));
-    asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(h1) : "f"(t1));
-    // Phi(x) = 1/2 + sign(x) (1/2 - h)  =>  x Phi(x) = x/2 + |x| (1/2 - h): no sign test, no select
-    const f32x2 half2 = pk2(0.5f, 0.5f);
-    const f32x2 xphi = fma2(ax, sub2(half2, pk2(h0, h1)), mul2(x, half2));
-    return mul2(a, xphi);
-}
 
 }  // namespace tc

@@ -27,8 +27,8 @@ __global__ void ncthw_to_cl_kernel(const float* __restrict__ x, __half* __restri
 
 // Tiled form for wide tensors (C % 64 == 0: the decoder's reference-frame feature maps, 128-512 channels): a 32-pixel x
 // 64-channel tile goes through shared memory, so the fp32 planes are read 128 bytes at a time AND the channels-last rows are
-// written as 16-byte vectors (the per-pixel loop above writes 2 bytes per thread per instruction: 460 GB/s, 1.7 ms of a
-// 47 ms decode, profiles/r02_vae_decode_launches.txt).  grid = (pixel tiles, channel tiles, B), 256 threads.
+// written as 16-byte vectors (the per-pixel loop above writes 2 bytes per thread per instruction).  grid = (pixel tiles,
+// channel tiles, B), 256 threads.
 __global__ void ncthw_to_cl_tiled_kernel(const float* __restrict__ x, __half* __restrict__ y, int C, long long thw, int Cpad,
                                          int coff, float scale) {
     tc::pdl_wait();

@@ -1,32 +1,23 @@
-// tooncrafter_b200 — implicit-GEMM convolution / linear layer on tcgen05 (sm_100a).
+// tooncrafter_b200 — implicit-GEMM convolution / linear layer on wgmma (sm_90a).
 //
-// One persistent, warp-specialised kernel serves every dense contraction of the UNet and the VAE decoder
-// (reference call sites listed in include/tooncrafter_b200.h):
+// One warp-specialised kernel serves every dense contraction of the UNet and the VAE decoder (reference call sites
+// listed in include/tooncrafter_b200.h).  One CTA computes one 128 x BN output tile (or one k-slice of it):
 //
-//   warp 0      TMA producer   : per k-block one 4-D box of the channels-last activation (im2col by
-//                                coordinate offset; out-of-bounds rows/cols are zero-filled by TMA == padding)
-//                                and one 2-D box of the [Cout][taps*C] weight matrix, 128B-swizzled.  Short-K launches
-//                                keep the whole weight N-tile resident in smem and stream only A.  A residual / skip
-//                                operand arrives as extra A-only k-blocks.
-//   warp 1      MMA issuer     : tcgen05.mma kind::f16, M=128 (cta_group::1) or M=256 (cta_group::2: two CTAs of a
-//                                cluster, each stages its own 128 A rows and half of the B tile), N=block_n, K=16, fp32
-//                                accumulators in TMEM, two buffers so the epilogue of tile i overlaps the mainloop of
-//                                i+1.  Residual k-blocks multiply by a 64x64 identity kept in smem (N=64 MMAs onto
-//                                accumulator columns [64r, 64r+64)): the skip add costs no epilogue instruction.
-//   warps 2..9  epilogue       : one output row per thread, 32-column chunks interleaved over two column groups;
-//                                tcgen05.ld (next chunk in flight) -> folded LayerNorm / bias / timestep embedding /
-//                                scale / GEGLU -> fp16 -> 64B-swizzled smem box -> TMA store (one 32x32 box per warp
-//                                where the tile geometry allows, else one 128x32 box per column group).  Optional
-//                                per-row {sum, sumsq} of the outputs for the consumer's LayerNorm fold.  Odd widths
-//                                (n_cols % 32 != 0, e.g. the 4-channel output conv) take the direct-store variant.
-//                                Short-K launches (epilogue-bound) stage ALL chunks of a tile and issue their TMA stores in
-//                                one burst behind a single proxy fence / barrier / commit.
-//   The producer and the issuer are single-thread loops (one elected lane runs the whole loop, waits included).
-//   Three instantiations of the epilogue (plain / GEGLU / direct-store) x {single CTA, CTA pair}; tile shape and pairing
-//   come from choose_tiles() (waves x per-tile cost with the tensor rate and the ~52 B/clk/SM L2->SM ingest bound).
+//   warpgroup 0    TMA producer  : one elected thread; per k-block one 4-D box of the channels-last activation (im2col
+//                                  by coordinate offset; out-of-bounds rows/cols are zero-filled by TMA == padding) and
+//                                  one 2-D box of the [Cout][taps*C] weight matrix, both 128B-swizzled, into a ring of
+//                                  `stages` shared-memory slots guarded by full / empty mbarriers.
+//   warpgroups 1-2 wgmma         : each owns 64 of the tile's 128 rows; m64n32k16 instructions over BN/32 column chunks,
+//                                  fp32 accumulators in registers, one k-block in flight behind the one being issued.
+//                                  After the last k-block the accumulators go to shared memory (the drained operand
+//                                  ring is reused), and the same 256 threads run the epilogue with one output row per
+//                                  thread and two column groups: folded LayerNorm / bias / timestep embedding / scale /
+//                                  residual or GEGLU -> fp16 -> 16-byte stores; optional per-row {sum, sumsq} of the
+//                                  outputs for the consumer's LayerNorm fold.
+//   split-K (few output tiles, long K loops): every slice parks its fp32 tile in a workspace, takes a ticket, and the
+//   last slice to arrive sums all slices in slice order (deterministic) and runs the epilogue.
 //
-// Roofline: tensor-bound for long K, L2-ingest-bound for 160-wide tiles, epilogue-issue-bound at K = 320 (profiles/);
-// algorithmic flops = 2 * M * n_cols * taps * C.
+// Algorithmic flops = 2 * M * n_cols * taps * C.
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -37,65 +28,28 @@ namespace {
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;                          // 64 halfs = one 128-byte swizzle row
 constexpr int kAStageBytes = kBlockM * kBlockK * 2;  // 16 KiB
-constexpr int kThreads = 320;  // warp 0 TMA, warp 1 MMA, warps 2..9 epilogue
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;  // TMEM column offset of the second accumulator
-
-// Division by a launch constant as multiply-high + shift (exact for dividends below 2^31): the per-tile coordinate
-// decode used ~10 generic integer divisions, 1000-2400 cycles of dependent latency per tile on the epilogue warps of
-// the short-K launches (in-kernel timeline, profiles/r02_gemm_epilogue_timeline.txt).
-struct FastDiv {
-    uint32_t d, mul, shr;
-};
-inline FastDiv make_fastdiv(uint32_t d) {
-    FastDiv f{d ? d : 1u, 0u, 0u};
-    uint32_t lg = 0;
-    while ((2u << lg) <= f.d && lg < 31) ++lg;                 // floor(log2 d)
-    f.shr = lg;
-    if ((f.d & (f.d - 1)) != 0)                                // not a power of two
-        f.mul = (uint32_t)((((unsigned long long)1 << (32 + lg)) + f.d - 1) / f.d);
-    return f;
-}
-__device__ __forceinline__ int fdiv(int n, const FastDiv& f) {
-    return (int)(f.mul ? (__umulhi((uint32_t)n, f.mul) >> f.shr) : ((uint32_t)n >> f.shr));
-}
+constexpr int kThreads = 384;                        // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
+constexpr int kEpiThreads = 256;
 
 struct alignas(64) GemmKParams {
     CUtensorMap tmA;
     CUtensorMap tmB;
-    CUtensorMap tmR;   // residual viewed as an A operand (res_kblocks > 0)
-    int res_kblocks;   // 0: residual (if any) is added in the epilogue from registers
-    CUtensorMap tmO;   // output, box {32 cols, TW, TH, TN}, 64B swizzle (tma_store != 0)
-    int tma_store;     // epilogue writes through shared memory + TMA stores (whole 32-column chunks)
-    CUtensorMap tmOw;  // output, per-warp box {32 cols, wbW, wbH, wbN} (warp_box != 0)
-    int warp_box;      // each epilogue warp's 32 rows form a box: per-warp TMA stores, no 128-thread barriers
-    float2* row_stats; // producer: per-row {sum, sumsq} partials, [M][row_stats_slots]
-    int row_stats_slots;
-    int ln_nslots;     // consumer: ln_stats holds [M][ln_nslots] partial sums, finished in the epilogue
-    float ln_eps, ln_inv_c;
-    int b_resident;    // the whole K extent of one B (weight) N-tile stays in shared memory across M tiles
     int taps;
     int tap_dx[TC_MAX_TAPS], tap_dy[TC_MAX_TAPS], tap_dn[TC_MAX_TAPS];
     int kc_per_tap;
     int TW, TH, TN;
     int oW, oH, oN;
-    int tiles_x, tiles_y, tiles_n;  // spatial tiling of the M dimension
-    int tiles_m, tiles_nn;          // tiles along M and along N
-    int BN;
-    int raster;                     // tile order, see TC_DECODE_TILE
-    FastDiv fd_nn, fd_mu, fd_x, fd_y, fd_xy, fd_b2;   // tiles_nn, M-tile units, tiles_x, tiles_y, tiles_x*tiles_y, bias2_rows_per
-    // split-K (long K loops on few output tiles, e.g. the 10x16 / 5x8 UNet levels where one wave of tiles leaves most SMs
-    // idle): work item = (tile, k-slice); every slice writes its fp32 partial tile to `ws_partial`, takes a ticket, and the
-    // LAST slice to arrive sums all partials in slice order (deterministic) and runs the normal epilogue
+    int tiles_x, tiles_y;           // spatial tiling of the M dimension
+    int tiles_nn;                   // tiles along N
+    int BN;                         // output columns per tile (GEGLU: value + gate columns)
     int ksplit, kb_per;             // k-slices per tile, k-blocks per slice
-    FastDiv fd_ks, fd_kc;           // ksplit, kc_per_tap
-    float* ws_partial;              // [total tiles][ksplit][128 rows][BN] floats
-    unsigned int* ws_ticket;        // [total tiles], zero between launches (the last slice resets it)
-    int stage_bufs;                 // output staging boxes per warp / column group (1; 2 in rotation; or one per chunk: batch_store)
-    int batch_store;                // short-K launches: all chunks of a tile are staged, then stored in one burst
+    float* ws_partial;              // [tiles][ksplit][128 rows][BNp] floats
+    unsigned int* ws_ticket;        // [tiles], zero between launches (the last slice resets it)
     int n_cols;
     int stages;
-    uint32_t a_bytes;  // bytes delivered per A box
+    uint32_t a_bytes;               // bytes delivered per A box
+    uint32_t b_bytes;               // bytes delivered per B box (BNp rows of 128 bytes)
+    uint32_t ring_bytes;            // operand ring (reused as the fp32 accumulator staging tile)
     __half* out;
     long long ldc;
     const float* bias;
@@ -105,1023 +59,369 @@ struct alignas(64) GemmKParams {
     const __half* res;
     long long ldr;
     float acc_scale;
-    int flags;
-    const float2* ln_stats;  // per output row {mean, rstd} (folded LayerNorm) or null
+    int geglu;
+    const float2* ln_stats;  // per output row {mean, rstd} (ln_nslots == 0) or [M][ln_nslots] partial {sum, sumsq}
     const float* ln_u;       // per column sum_k Wt[j][k]
+    int ln_nslots;
+    float ln_eps, ln_inv_c;
+    float2* row_stats;       // producer: per-row {sum, sumsq} partials, [M][row_stats_slots]
+    int row_stats_slots;
 };
 
-// Profiling modes (tc_debug_set_gemm_mode) are honoured by TRACE builds only (TC_BUILD_TRACE=1, loaded through TC_LIB_PATH):
-// the production kernels do not read the mode word — it was a global load at the head of every tile's epilogue.
-#if defined(TC_GEMM_TRACE) && TC_GEMM_TRACE
-#define TC_DEBUG_MODE() g_tc_gemm_debug
-#else
-#define TC_DEBUG_MODE() 0
-#endif
-__device__ int g_tc_gemm_debug = 0;   // profiling aid (scripts/prof_epilogue.py): 1 = no global stores, 2 = no epilogue body,
-                                      // 4 = record per-tile clock64() stamps of each warp role (scripts/trace_gemm.py)
-#if defined(TC_GEMM_TRACE) && TC_GEMM_TRACE
-constexpr int kTraceTiles = 32, kTraceSlots = 16, kTraceCtas = 160;
-__device__ unsigned long long g_tc_gemm_trace[kTraceCtas * kTraceTiles * kTraceSlots];
-#endif
-// compiled in only with -DTC_GEMM_TRACE=1 (python tooncrafter_b200/build.py --trace): even the disabled checks cost the
-// long-K convolutions 10-25 % (measured, scripts/ab_conv.py)
-#if defined(TC_GEMM_TRACE) && TC_GEMM_TRACE
-#define TC_TRACE(slot, ti)                                                                                   \
-    if ((g_tc_gemm_debug & 4) && (ti) < kTraceTiles && blockIdx.x < kTraceCtas)                                \
-        g_tc_gemm_trace[((int)blockIdx.x * kTraceTiles + (ti)) * kTraceSlots + (slot)] = (unsigned long long)clock64();
-#else
-#define TC_TRACE(slot, ti)
-#endif
-
-__device__ __forceinline__ void store_row16(__half* dst, const float (&v)[16], int ncols_valid) {
-    if (TC_DEBUG_MODE() & 1) return;
-    if (ncols_valid >= 16) {
-        uint4 u0, u1;
-        __half2 h[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) h[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-        u0.x = *reinterpret_cast<uint32_t*>(&h[0]);
-        u0.y = *reinterpret_cast<uint32_t*>(&h[1]);
-        u0.z = *reinterpret_cast<uint32_t*>(&h[2]);
-        u0.w = *reinterpret_cast<uint32_t*>(&h[3]);
-        u1.x = *reinterpret_cast<uint32_t*>(&h[4]);
-        u1.y = *reinterpret_cast<uint32_t*>(&h[5]);
-        u1.z = *reinterpret_cast<uint32_t*>(&h[6]);
-        u1.w = *reinterpret_cast<uint32_t*>(&h[7]);
-        reinterpret_cast<uint4*>(dst)[0] = u0;
-        reinterpret_cast<uint4*>(dst)[1] = u1;
-    } else {
-#pragma unroll
-        for (int i = 0; i < 16; ++i)
-            if (i < ncols_valid) dst[i] = __float2half_rn(v[i]);
-    }
+__device__ __forceinline__ uint32_t pack_h2(float x, float y) {
+    __half2 h = __floats2half2_rn(x, y);
+    return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// kPair = true: two CTAs of a cluster form one tcgen05 cta_group::2 pair (M = 256 per MMA, each CTA loads its own 128
-// A rows and HALF of the B tile), which cuts the shared-memory/L2 operand traffic per MAC by ~30-45 % — the single-CTA
-// kernel saturates at ~62 B/clk/SM of TMA ingest (profiles/r01_*conv320*).
-// kEpi: 0 = TMA-store epilogue, 1 = TMA-store GEGLU epilogue, 2 = legacy epilogue (direct 16-byte / scalar stores for
-// odd widths); separate instantiations keep each variant's register footprint below the 168-register cap
-template <bool kPair, int kEpi>
+// kNJ = BNp / 32: column chunks of one m64n32k16 accumulator each (BNp = BN rounded up to 32)
+template <int kNJ>
 __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_constant__ GemmKParams p) {
     tc::pdl_launch_dependents();   // the successor's prologue may overlap this kernel; it blocks in its own pdl_wait
+    constexpr int kBNp = kNJ * 32;
+    constexpr int kLds = kBNp + 4;  // staging row stride in floats (rows 4 banks apart)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
-    const int warp = threadIdx.x >> 5;
-    const int lane = threadIdx.x & 31;
     const int S = p.stages;
     const int BN = p.BN;
-    const uint32_t rank = kPair ? tc::cluster_ctarank() : 0u;      // 0 = leader (issues the MMAs)
-    const int b_rows = kPair ? (BN >> 1) : BN;                      // B rows staged by THIS CTA
-    const uint32_t b_stage_bytes = (uint32_t)b_rows * 128u;
-
-    const int main_kblocks = p.taps * p.kc_per_tap;
     uint8_t* sA = smem;
     uint8_t* sB = smem + (size_t)S * kAStageBytes;
-    // B ring (one slot per stage) or, b_resident, one slot per k-block of the N tile
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(sB + (size_t)(p.b_resident ? main_kblocks : S) * b_stage_bytes);
+    float* stg = reinterpret_cast<float*>(smem);   // [128][kLds] fp32 accumulators, after the ring has drained
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.ring_bytes);
     uint64_t* empty_bar = full_bar + S;
-    uint64_t* tfull_bar = empty_bar + S;   // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;  // [2]
-    uint64_t* bfull_bar = tempty_bar + 2;  // resident B loaded
-    uint64_t* bfree_bar = bfull_bar + 1;   // every MMA reading the resident B has retired
-    uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bfree_bar + 1);
-    // epilogue staging of the per-column vectors (bias, folded-LayerNorm u): [2 accumulators][bias 256 | u 256] floats
-    int* s_flag = reinterpret_cast<int*>(tmem_ptr_smem + 1);     // split-K: "this CTA holds the last slice of the tile"
-    float* s_epi = reinterpret_cast<float*>(tmem_ptr_smem + 4);
-    // output staging for the TMA-store epilogue: one 128-row x 32-column (64 B, 64B-swizzled) box per column group
-    uint8_t* s_stage = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(s_epi + 1024) + 1023) & ~uintptr_t(1023));
-    // 64 x 64 identity (K-major, 128B-swizzled like a weight tile): the B operand of the residual k-blocks
-    uint8_t* s_eye = s_stage + (size_t)p.stage_bufs * 16384;   // one or two staging boxes (16 KiB each) in rotation
-    // producer-side row statistics: column group 1 hands its partials to group 0 (two buffers by tile parity)
-    float2* s_rs = reinterpret_cast<float2*>(s_eye + 8192);
+    float* s_bias = reinterpret_cast<float*>(empty_bar + S);   // [256]
+    float* s_u = s_bias + 256;                                 // [256]
+    float2* s_rs = reinterpret_cast<float2*>(s_u + 256);       // [128] row statistics of column group 1
+    int* s_flag = reinterpret_cast<int*>(s_rs + 128);
 
-    if (warp == 0 && lane == 0) {
+    const int tid = threadIdx.x;
+    if (tid == 0) {
         tc::tma_prefetch_desc(&p.tmA);
         tc::tma_prefetch_desc(&p.tmB);
-        if (p.res_kblocks) {
-            tc::tma_prefetch_desc(&p.tmR);
-        }
-        if (p.tma_store) tc::tma_prefetch_desc(p.warp_box ? &p.tmOw : &p.tmO);
-    }
-    if (warp == 1 && lane == 0) {
         for (int s = 0; s < S; ++s) {
             tc::mbar_init(&full_bar[s], 1);
-            tc::mbar_init(&empty_bar[s], 1);
+            tc::mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
         }
-        for (int a = 0; a < 2; ++a) {
-            tc::mbar_init(&tfull_bar[a], 1);
-            tc::mbar_init(&tempty_bar[a], kPair ? 16 : 8);   // epilogue warps of both CTAs release the leader
-        }
-        tc::mbar_init(bfull_bar, 1);
-        tc::mbar_init(bfree_bar, 1);
         tc::fence_mbar_init();
     }
-    if (warp == 2) {
-        if constexpr (kPair) {
-            tc::tmem_alloc_pair(tmem_ptr_smem, kTmemCols);
-            tc::tmem_relinquish_pair();
-        } else {
-            tc::tmem_alloc(tmem_ptr_smem, kTmemCols);
-            tc::tmem_relinquish();
-        }
-    }
-    if (p.res_kblocks && warp >= 2) {
-        // this CTA's rows of the identity: a pair splits B by rows (32 each), a single CTA holds all 64
-        const int e = (int)threadIdx.x - 64;                       // 0..255
-        const int rows = kPair ? 32 : 64;
-        for (int i = e; i < rows * 8; i += 256) reinterpret_cast<uint4*>(s_eye)[i] = make_uint4(0u, 0u, 0u, 0u);
-        asm volatile("bar.sync 1, 256;" ::: "memory");
-        if (e < rows) {
-            const int k = (kPair ? (int)rank * 32 : 0) + e;        // column holding the 1 of local row e
-            *reinterpret_cast<__half*>(s_eye + e * 128 + (((k >> 3) ^ (e & 7)) << 4) + (k & 7) * 2) = __float2half(1.f);
-        }
-        tc::fence_proxy_async_smem();
-    }
-    tc::tc_fence_before();
-    if constexpr (kPair) tc::cluster_sync_all(); else __syncthreads();
-    tc::tc_fence_after();
-    const uint32_t tmem_base = *tmem_ptr_smem;
-    // barriers, TMEM and the identity tile are set up: from here on the kernel touches its predecessors' results
+    __syncthreads();
     tc::pdl_wait();
 
-    // work units: a single CTA takes one M tile, a CTA pair takes two consecutive M tiles (rank selects which)
-    const int unit = kPair ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-    const int n_units = kPair ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-    const int tiles_mu = kPair ? ((p.tiles_m + 1) >> 1) : p.tiles_m;
-    const int tiles_mp = tiles_mu * (kPair ? 2 : 1);             // M tiles incl. the odd tail of a pair (workspace stride)
-    const int total_tiles = tiles_mu * p.tiles_nn * p.ksplit;   // work items: (output tile, k-slice), slice fastest
-    // work item -> output tile and the k-blocks of its slice (slice 0 also takes the residual k-blocks)
-#define TC_DECODE_WORK(wi)                                                          \
-    const int tile = fdiv((wi), p.fd_ks);                                           \
-    const int ks = (wi) - tile * p.ksplit;                                          \
-    const int kb_begin = ks * p.kb_per;                                             \
-    const int kb_end = (kb_begin + p.kb_per < main_kblocks) ? kb_begin + p.kb_per : main_kblocks; \
-    const int res_kb = (ks == 0) ? p.res_kblocks : 0;
-    // tile -> (nt, mt) for this CTA; mt >= tiles_m (odd tail of a pair) decodes to out-of-range coordinates:
-    // its TMA boxes are zero-filled and its rows are never stored
-    // raster 0: N-tile-major (all M tiles of weight tile 0, then tile 1, ...: the resident-weight order);
-    // raster 1: N tile fastest — the CTAs that run side by side work on the SAME rows of A with different weight tiles,
-    // so A comes from DRAM once and from L2 for the other N tiles (the N-major order streamed the 100-200 MB A operand
-    // of the FF2 GEMMs once per N tile: 2-3.3x DRAM traffic, profiles/r01_unet_b2_launches_final.txt).  The host makes
-    // the number of work units a multiple of tiles_nn when the weights are resident, so a CTA's N tile never changes.
-#define TC_TILE_NT(tile) (p.raster ? (tile) - fdiv((tile), p.fd_nn) * p.tiles_nn : fdiv((tile), p.fd_mu))
-#define TC_DECODE_TILE(tile)                                                   \
-    const int nt = TC_TILE_NT(tile);                                           \
-    const int mtu_ = p.raster ? fdiv((tile), p.fd_nn) : (tile) - nt * tiles_mu;  \
-    const int mt = mtu_ * (kPair ? 2 : 1) + (int)rank;                         \
-    const int mtx_ = fdiv(mt, p.fd_x);                                         \
-    const int tx = mt - mtx_ * p.tiles_x;                                      \
-    const int tn = fdiv(mt, p.fd_xy);                                          \
-    const int ty = mtx_ - tn * p.tiles_y;
+    // work item -> (tile, k-slice); tile -> (N tile fastest, M tile): CTAs that run side by side share rows of A
+    const int wi = (int)blockIdx.x;
+    const int tile = wi / p.ksplit;
+    const int ks = wi - tile * p.ksplit;
+    const int nt = tile % p.tiles_nn;
+    const int mt = tile / p.tiles_nn;
+    const int tx = mt % p.tiles_x;
+    const int ty = (mt / p.tiles_x) % p.tiles_y;
+    const int tn = mt / (p.tiles_x * p.tiles_y);
+    const int main_kblocks = p.taps * p.kc_per_tap;
+    const int kb_begin = ks * p.kb_per;
+    const int kb_end = min(kb_begin + p.kb_per, main_kblocks);
 
-    if (warp == 0) {
+    if (tid < 128) {
         // ------------------------------------------------------------------ TMA producer
-        // ONE elected lane runs the whole loop, waits included (like the MMA issuer below).  A plain `if (lane == 0)` makes
-        // the issue code thread-divergent and ptxas wraps every TMA / MMA in ELECT + R2UR.BROADCAST + BRA.U.ANY sequences
-        // (measured: ~550 cycles of issue latency per k-block, the kernel's bottleneck in profiles/r01_*conv320*).
-        if (tc::elect_one()) {
+        if (tid < 32 && tc::elect_one()) {
+            const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = tn * p.TN;
             int stage = 0;
             uint32_t phase = 0;
-            int cur_nt = -1;
-            uint32_t bphase = 0;
-            int ti = 0;
-            for (int wi = unit; wi < total_tiles; wi += n_units, ++ti) {
-                TC_DECODE_WORK(wi)
-                TC_DECODE_TILE(tile)
-                const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = tn * p.TN;
-                TC_TRACE(0, ti)
-                if (p.b_resident && nt != cur_nt) {
-                    // (re)load the weight N-tile: skinny GEMMs (M >> N, short K) otherwise re-fetch it from L2 for every
-                    // M tile, which is more traffic than A itself and runs into the ~6300 B/clk chip-wide L2 cap
-                    tc::mbar_wait(bfree_bar, bphase ^ 1u);
-                    const uint32_t bytes = (uint32_t)main_kblocks * b_stage_bytes;
-                    if constexpr (kPair) {
-                        if (rank == 0) tc::mbar_arrive_expect_tx(bfull_bar, 2u * bytes);
-                        for (int kb = 0; kb < main_kblocks; ++kb)
-                            tc::tma_load_2d_pair(sB + (size_t)kb * b_stage_bytes, &p.tmB, bfull_bar, kb * kBlockK,
-                                                 nt * BN + (int)rank * b_rows);
-                    } else {
-                        tc::mbar_arrive_expect_tx(bfull_bar, bytes);
-                        for (int kb = 0; kb < main_kblocks; ++kb)
-                            tc::tma_load_2d(sB + (size_t)kb * b_stage_bytes, &p.tmB, bfull_bar, kb * kBlockK, nt * BN);
-                    }
-                    cur_nt = nt;
-                    bphase ^= 1u;
-                }
-                const uint32_t bytes = p.a_bytes + (p.b_resident ? 0u : b_stage_bytes);
-                int tap = fdiv(kb_begin, p.fd_kc);
-                int kc = kb_begin - tap * p.kc_per_tap;
-                for (int kb = kb_begin; kb < kb_end; ++kb) {
-                    const int ax = x0 + p.tap_dx[tap], ay = y0 + p.tap_dy[tap], an = n0 + p.tap_dn[tap];
-                    tc::mbar_wait(&empty_bar[stage], phase ^ 1u);
-                    uint8_t* dA = sA + (size_t)stage * kAStageBytes;
-                    uint8_t* dB = sB + (size_t)stage * b_stage_bytes;
-                    const int kcol = kb * kBlockK;               // == (tap * kc_per_tap + kc) * 64
-                    if constexpr (kPair) {
-                        // both CTAs' bytes are credited to the leader's barrier
-                        if (rank == 0) tc::mbar_arrive_expect_tx(&full_bar[stage], 2u * bytes);
-                        tc::tma_load_4d_pair(dA, &p.tmA, &full_bar[stage], kc * kBlockK, ax, ay, an);
-                        if (!p.b_resident)
-                            tc::tma_load_2d_pair(dB, &p.tmB, &full_bar[stage], kcol, nt * BN + (int)rank * b_rows);
-                    } else {
-                        tc::mbar_arrive_expect_tx(&full_bar[stage], bytes);
-                        tc::tma_load_4d(dA, &p.tmA, &full_bar[stage], kc * kBlockK, ax, ay, an);
-                        if (!p.b_resident) tc::tma_load_2d(dB, &p.tmB, &full_bar[stage], kcol, nt * BN);
-                    }
-                    if (++kc == p.kc_per_tap) { kc = 0; ++tap; }
-                    if (++stage == S) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                // residual as extra k-blocks: acc[:, 64r:64r+64] += R[tile rows][64r:64r+64] @ I64  (TMA-coalesced, fully
-                // async; loading it from registers in the epilogue cost 32 us of a 81 us launch at M=81920, N=K=320)
-                for (int r = 0; r < res_kb; ++r) {
-                    tc::mbar_wait(&empty_bar[stage], phase ^ 1u);
-                    uint8_t* dA = sA + (size_t)stage * kAStageBytes;   // A slot only: B is the resident identity
-                    if constexpr (kPair) {
-                        if (rank == 0) tc::mbar_arrive_expect_tx(&full_bar[stage], 2u * p.a_bytes);
-                        tc::tma_load_4d_pair(dA, &p.tmR, &full_bar[stage], nt * BN + r * kBlockK, x0, y0, n0);
-                    } else {
-                        tc::mbar_arrive_expect_tx(&full_bar[stage], p.a_bytes);
-                        tc::tma_load_4d(dA, &p.tmR, &full_bar[stage], nt * BN + r * kBlockK, x0, y0, n0);
-                    }
-                    if (++stage == S) {
-                        stage = 0;
-                        phase ^= 1u;
-                    }
-                }
-                TC_TRACE(1, ti)
+            int tap = kb_begin / p.kc_per_tap;
+            int kc = kb_begin - tap * p.kc_per_tap;
+            for (int kb = kb_begin; kb < kb_end; ++kb) {
+                tc::mbar_wait(&empty_bar[stage], phase ^ 1u);
+                tc::mbar_arrive_expect_tx(&full_bar[stage], p.a_bytes + p.b_bytes);
+                tc::tma_load_4d(sA + (size_t)stage * kAStageBytes, &p.tmA, &full_bar[stage], kc * kBlockK,
+                                x0 + p.tap_dx[tap], y0 + p.tap_dy[tap], n0 + p.tap_dn[tap]);
+                tc::tma_load_2d(sB + (size_t)stage * p.b_bytes, &p.tmB, &full_bar[stage], kb * kBlockK, nt * BN);
+                if (++kc == p.kc_per_tap) { kc = 0; ++tap; }
+                if (++stage == S) { stage = 0; phase ^= 1u; }
             }
         }
-        __syncwarp();
-    } else if (warp == 1) {
-        // ------------------------------------------------------------------ MMA issuer
-        // ONE elected lane runs the whole loop (waits included): issuing is the bottleneck of the narrow tiles — a k-block of
-        // four M256 x N160 MMAs executes in 320 cycles but took ~475 to issue when the warp walked the loop converged and
-        // elected a lane per k-block (ELECT / BSSY / WARPSYNC and 64-bit descriptor arithmetic on vector registers feeding
-        // R2UR per k-block; in-kernel timeline profiles/r02_gemm_trace_k320.txt).  Descriptors advance by 32-bit adds on
-        // their low words (start-address field, no carry: shared memory is < 256 KiB), main and residual k-blocks have
-        // their own loops.
-        if (rank == 0) {
-            if (tc::elect_one()) {
-                const uint32_t idesc = tc::umma_idesc_f16(kPair ? 2 * kBlockM : kBlockM, (uint32_t)BN, 0, 0);
-                const uint32_t idesc_eye = tc::umma_idesc_f16(kPair ? 2 * kBlockM : kBlockM, 64u, 0, 0);
-                const uint64_t a_desc0 = tc::umma_desc_sw128(tc::smem_u32(sA));
-                const uint64_t b_desc0 = tc::umma_desc_sw128(tc::smem_u32(sB));
-                const uint64_t eye_desc = tc::umma_desc_sw128(tc::smem_u32(s_eye));
-                const uint32_t a_lo0 = (uint32_t)a_desc0, a_hi = (uint32_t)(a_desc0 >> 32);
-                const uint32_t b_lo0 = (uint32_t)b_desc0, b_hi = (uint32_t)(b_desc0 >> 32);
-                const uint32_t a_step = (uint32_t)(kAStageBytes >> 4), b_step = b_stage_bytes >> 4;
-                auto mk = [](uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | (uint64_t)lo; };
-                int stage = 0;
-                uint32_t phase = 0;
-                int acc = 0;
-                uint32_t acc_phase = 0;
-                int cur_nt = -1;
-                uint32_t bphase = 0;
-                int ti = 0;
-                for (int wi = unit; wi < total_tiles; wi += n_units, ++ti) {
-                    TC_DECODE_WORK(wi)
-                    const int n_main = kb_end - kb_begin;
-                    if (p.b_resident && TC_TILE_NT(tile) != cur_nt) {
-                        tc::mbar_wait(bfull_bar, bphase);
-                        bphase ^= 1u;
-                        cur_nt = TC_TILE_NT(tile);
-                    }
-                    tc::mbar_wait(&tempty_bar[acc], acc_phase ^ 1u);
-                    tc::tc_fence_after();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)acc * kAccStride;
-                    TC_TRACE(2, ti)
-                    for (int kb = 0; kb < n_main; ++kb) {
-                        tc::mbar_wait(&full_bar[stage], phase);
-                        tc::tc_fence_after();
-                        if (kb == 0) { TC_TRACE(3, ti) }
-                        const uint32_t a_lo = a_lo0 + a_step * (uint32_t)stage;
-                        const uint32_t b_lo = b_lo0 + b_step * (uint32_t)(p.b_resident ? kb : stage);
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k) {
-                            // advance 16 halfs = 32 bytes inside the swizzle row: +2 in the (addr >> 4) field
-                            if constexpr (kPair)
-                                tc::umma_f16_pair(d_tmem, mk(a_lo + 2u * k, a_hi), mk(b_lo + 2u * k, b_hi), idesc, (kb | k) != 0 ? 1u : 0u);
-                            else
-                                tc::umma_f16(d_tmem, mk(a_lo + 2u * k, a_hi), mk(b_lo + 2u * k, b_hi), idesc, (kb | k) != 0 ? 1u : 0u);
-                        }
-                        if constexpr (kPair) tc::umma_commit_pair(&empty_bar[stage]); else tc::umma_commit(&empty_bar[stage]);
-                        if (++stage == S) {
-                            stage = 0;
-                            phase ^= 1u;
-                        }
-                    }
-                    // residual k-blocks: N = 64 identity MMAs onto accumulator columns [64 r, 64 r + 64)
-                    for (int r = 0; r < res_kb; ++r) {
-                        tc::mbar_wait(&full_bar[stage], phase);
-                        tc::tc_fence_after();
-                        const uint32_t a_lo = a_lo0 + a_step * (uint32_t)stage;
-                        const uint32_t dcol = d_tmem + (uint32_t)(r * 64);
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k) {
-                            if constexpr (kPair)
-                                tc::umma_f16_pair(dcol, mk(a_lo + 2u * k, a_hi), eye_desc + (uint64_t)(k * 2), idesc_eye, (n_main | k) != 0 ? 1u : 0u);
-                            else
-                                tc::umma_f16(dcol, mk(a_lo + 2u * k, a_hi), eye_desc + (uint64_t)(k * 2), idesc_eye, (n_main | k) != 0 ? 1u : 0u);
-                        }
-                        if constexpr (kPair) tc::umma_commit_pair(&empty_bar[stage]); else tc::umma_commit(&empty_bar[stage]);
-                        if (++stage == S) {
-                            stage = 0;
-                            phase ^= 1u;
-                        }
-                    }
-                    if constexpr (kPair) tc::umma_commit_pair(&tfull_bar[acc]); else tc::umma_commit(&tfull_bar[acc]);
-                    // last tile on this weight N-tile: tell the producer(s) when its MMAs have drained
-                    const int next = wi + n_units;        // (weights are only resident without split-K: work item == tile)
-                    if (p.b_resident && next < total_tiles && TC_TILE_NT(next) != cur_nt) {
-                        if constexpr (kPair) tc::umma_commit_pair(bfree_bar); else tc::umma_commit(bfree_bar);
-                    }
-                    TC_TRACE(4, ti)
-                    acc ^= 1;
-                    if (acc == 0) acc_phase ^= 1u;
-                }
-            }
-            __syncwarp();
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue (warps 2..9)
-        // Two warps per TMEM lane quadrant: "column group" 0 takes the first half of the tile's columns, group 1 the
-        // second half, so 256 threads keep loads/stores in flight.  Each thread owns one output row; the residual
-        // slice of its row is prefetched into registers BEFORE waiting for the accumulator, i.e. it is hidden
-        // behind the tile's own mainloop.
-        const int q = warp & 3;             // TMEM lane quadrant this warp may access
-        const int cg = (warp - 2) >> 2;     // column group 0 / 1
-        const int row = q * 32 + lane;
-        const int rx = row % p.TW;
-        const int ry = (row / p.TW) % p.TH;
-        const int rn = row / (p.TW * p.TH);
-        const bool geglu = kEpi == 1 || (kEpi == 2 && (p.flags & TC_EPI_GEGLU) != 0);
-        const int width = geglu ? (BN >> 1) : BN;                   // output columns per tile
-        const int split = ((width / 16 + 1) / 2) * 16;              // group 0: [0, split), group 1: [split, width)
-        const int c_begin = cg == 0 ? 0 : split;
-        const int c_end = cg == 0 ? split : width;
-        const bool vec_ok = (p.n_cols % 16) == 0;                   // all chunks complete -> 16-byte paths
-        // TMA-store path: 32-column chunks, chunk k belongs to column group k & 1
-        // staging: one 128-row box per column group, or (warp_box) one 32-row box per warp
-        const bool warp_box = p.warp_box != 0;
-        uint8_t* stg = warp_box ? s_stage + (warp - 2) * 2048 : s_stage + cg * 8192;
-        // the warp that issues this thread's TMA stores (warp-uniform); the issuing LANE is picked with elect.sync at each
-        // use: behind a per-lane predicate (lane == 0) ptxas emits the store as a divergent R2UR / BRA.U.ANY loop — ~320
-        // cycles per chunk in the in-kernel timeline (profiles/r02_gemm_trace_k320.txt), as it did for the TMA loads in round 1
-        const bool store_warp = warp_box ? true : (warp == 2 + 4 * cg);
-        const uint32_t stg_row = tc::smem_u32(stg) + (uint32_t)(warp_box ? lane : row) * 64u;
-        const uint32_t stg_swz = (uint32_t)((row >> 1) & 3);
-        // first row of this warp inside the tile box (warp_box: the origin of its store box)
-        const int wx = (q * 32) % p.TW, wy = ((q * 32) / p.TW) % p.TH, wn = (q * 32) / (p.TW * p.TH);
-        const bool warp_rows_in_tile = q * 32 < p.TW * p.TH * p.TN;
-        int staged_nt = -1, sb = 1;
-        uint32_t n_stores = 0;   // TMA-store chunks issued so far by this warp / column group: picks the staging box
-        int acc = 0;
-        uint32_t acc_phase = 0;
-        int ti = 0;
-        // {mean, rstd} of output row m for the LayerNorm folded into this GEMM (1, 0 without one)
-        auto ln_row_stats = [&](bool ok, long long mrow, float& mean, float& rstd) {
-            mean = 0.f;
-            rstd = 1.f;
-            if (!p.ln_stats || !ok) return;
-            if (p.ln_nslots > 0) {
-                // partial {sum, sumsq} slots written by the producer GEMM's epilogue (fixed order: deterministic)
-                float s1 = 0.f, s2 = 0.f;
-                const float2* ps = p.ln_stats + mrow * p.ln_nslots;
-#pragma unroll 4
-                for (int i = 0; i < p.ln_nslots; ++i) {
-                    const float2 st = __ldg(ps + i);
-                    s1 += st.x;
-                    s2 += st.y;
-                }
-                mean = s1 * p.ln_inv_c;
-                const float var = fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f);
-                rstd = rsqrtf(var + p.ln_eps);
-            } else {
-                const float2 st = __ldg(p.ln_stats + mrow);
-                mean = st.x;
-                rstd = st.y;
-            }
-        };
-        float ln_mean = 0.f, ln_rstd = 1.f;
-        float2 pre[4];                                     // next tile's partial slots (ln_nslots <= 4), raw
-        const bool pre_ok = p.ln_stats != nullptr && p.ln_nslots >= 1 && p.ln_nslots <= 4;
-        bool pre_row_ok = false;
-        for (int wi = unit; wi < total_tiles; wi += n_units, ++ti) {
-            TC_DECODE_WORK(wi)
-            (void)kb_begin; (void)kb_end; (void)res_kb;
-            TC_DECODE_TILE(tile)
-            const int x = tx * p.TW + rx, y = ty * p.TH + ry, n = tn * p.TN + rn;
-            const bool row_ok = (rn < p.TN) && (x < p.oW) && (y < p.oH) && (n < p.oN);
-            const long long m = ((long long)n * p.oH + y) * p.oW + x;
-            const __half* rrow = (p.res && p.res_kblocks == 0 && row_ok) ? p.res + m * p.ldr + (long long)nt * BN : nullptr;
+        return;
+    }
 
-            // folded-LayerNorm row statistics: loaded one tile ahead (below, after the accumulator wait), so their L2 round
-            // trip hides behind this tile's epilogue instead of heading the next one (4.6 % of the samples of the GEGLU
-            // launch sat on the first use of these loads)
-            if (ti == 0 || !pre_ok) {
-                ln_row_stats(row_ok, m, ln_mean, ln_rstd);
-            } else {
-                // finish the partials fetched during the previous tile (only now are the loaded values touched)
-                const float s1 = (pre[0].x + pre[1].x) + (pre[2].x + pre[3].x), s2 = (pre[0].y + pre[1].y) + (pre[2].y + pre[3].y);
-                ln_mean = s1 * p.ln_inv_c;
-                ln_rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - ln_mean * ln_mean, 0.f) + p.ln_eps);
-                if (!pre_row_ok) { ln_mean = 0.f; ln_rstd = 1.f; }
-            }
-            const float ln_rm = -ln_rstd * ln_mean;
-            // ---- residual prefetch (up to 128 columns = 16 x 16 B per thread)
-            uint4 rres[16];
-            if (kEpi == 2 && rrow && vec_ok) {
+    // ---------------------------------------------------------------------- MMA warpgroups
+    const int et = tid - 128;                 // 0..255
+    const int wg = et >> 7;                   // rows [64 wg, 64 wg + 64)
+    const int warp = (et >> 5) & 3, lane = et & 31;
+    {
+        // per-column vectors of this N tile (zeros when the launch has none): the epilogue runs one branch-free form
+        const int col = nt * BN + et;
+        const bool ok = et < BN && col < p.n_cols;
+        s_bias[et] = (ok && p.bias) ? __ldg(p.bias + col) : 0.f;
+        s_u[et] = (ok && p.ln_u) ? __ldg(p.ln_u + col) : 0.f;
+    }
+    float acc[kNJ][16];
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const int c = c_begin + j * 8;
-                    if (c < c_end && nt * BN + c < p.n_cols) rres[j] = *reinterpret_cast<const uint4*>(rrow + c);
-                }
-            }
-
-            // ---- per-column vectors of this N tile -> smem, (re)staged only when the N tile changes (global latency
-            // hidden behind the tile's mainloop; reading them with __ldg after the TMEM load put an L2 round trip on
-            // every 16-column chunk: profiles/r01_ncu_lin320).  Two buffers: a warp that runs ahead writes the other one.
-            const bool restage = nt != staged_nt;
-            if (restage) {
-                sb ^= 1;
-                staged_nt = nt;
-                float* wb = s_epi + sb * 512;
-                const int e = (int)threadIdx.x - 64;            // 0..255 over the 8 epilogue warps
-                const int col = nt * BN + e;
-                const bool ok = e < BN && col < p.n_cols;
-                // both vectors are always defined (zeros when the launch has no bias / no folded LayerNorm): the TMA-store
-                // epilogues then run ONE branch-free form,  rstd * acc + (rm * u + bias)  with rstd = 1, rm = 0 by default
-                wb[e] = (ok && p.bias) ? __ldg(p.bias + col) : 0.f;
-                wb[256 + e] = (ok && p.ln_u) ? __ldg(p.ln_u + col) : 0.f;
-            }
-            float* sbias = s_epi + sb * 512;
-            float* su = sbias + 256;
-            const uint32_t sbias_a = tc::smem_u32(sbias);          // u lives 1024 bytes (256 floats) behind the bias
-
-            if (threadIdx.x == 64) { TC_TRACE(5, ti) }
-            tc::mbar_wait(&tfull_bar[acc], acc_phase);
-            tc::tc_fence_after();
-            if (threadIdx.x == 64) { TC_TRACE(6, ti) }
-            if (restage) asm volatile("bar.sync 1, 256;" ::: "memory");       // staging visible to all epilogue warps
-            if (pre_ok && wi + n_units < total_tiles) {      // (folded LayerNorm launches never split K: work item == tile)
-                const int tile2 = wi + n_units;
-                const int nt2 = TC_TILE_NT(tile2);
-                const int mtu2 = p.raster ? fdiv(tile2, p.fd_nn) : tile2 - nt2 * tiles_mu;
-                const int mt2 = mtu2 * (kPair ? 2 : 1) + (int)rank;
-                const int mtx2 = fdiv(mt2, p.fd_x), tn2 = fdiv(mt2, p.fd_xy);
-                const int x2 = (mt2 - mtx2 * p.tiles_x) * p.TW + rx, y2 = (mtx2 - tn2 * p.tiles_y) * p.TH + ry;
-                const int n2 = tn2 * p.TN + rn;
-                pre_row_ok = (rn < p.TN) && (x2 < p.oW) && (y2 < p.oH) && (n2 < p.oN);
-                const float2* ps = p.ln_stats + (((long long)n2 * p.oH + y2) * p.oW + x2) * p.ln_nslots;
-                // volatile asm: the compiler otherwise sinks these loads to their first use at the top of the next tile
-                // (4.4 % of the samples of the GEGLU launch sat there: profiles/r02_ncu_gemm_geglu_insitu.txt)
+    for (int j = 0; j < kNJ; ++j)
 #pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    pre[i] = make_float2(0.f, 0.f);
-                    if (pre_row_ok && i < p.ln_nslots)
-                        asm volatile("ld.global.nc.v2.f32 {%0, %1}, [%2];" : "=f"(pre[i].x), "=f"(pre[i].y) : "l"(ps + i));
-                }
-            }
-            if (threadIdx.x == 64) { TC_TRACE(15, ti) }
-            const uint32_t taddr = tmem_base + (uint32_t)acc * kAccStride + ((uint32_t)(q * 32) << 16);
-
-            // ---- split-K: park this slice's fp32 accumulator tile, release TMEM, take a ticket; only the last slice of
-            // the tile to arrive goes on (it sums the slices in slice order: deterministic whatever the arrival order)
-            bool reduce = false, run_epilogue = true;
-            if (kEpi == 0 && p.ksplit > 1) {
-                // parked layout: [tile][slice][32-column chunk][4-float group 0..7][row 0..127] x 4 floats — the 32 rows of a
-                // warp write 512 contiguous bytes per instruction (row-major would touch 32 lines per instruction)
-                uint4* wslice = reinterpret_cast<uint4*>(p.ws_partial + ((long long)(nt * tiles_mp + mt) * p.ksplit + ks) * kBlockM * BN) + row;
-#pragma unroll 1
-                for (int jc = 0; jc < 4; ++jc) {
-                    const int c = (cg + 2 * jc) * 32;
-                    if (c >= BN) break;
-                    uint32_t r[32];
-                    tc::tmem_ld32(taddr + (uint32_t)c, r);
-                    tc::tmem_ld_wait();
+        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+    {
+        const uint64_t a_desc0 = tc::wgmma_desc_sw128(tc::smem_u32(sA + wg * 64 * 128));
+        const uint64_t b_desc0 = tc::wgmma_desc_sw128(tc::smem_u32(sB));
+        int stage = 0, prev = -1;
+        uint32_t phase = 0;
+        for (int kb = kb_begin; kb < kb_end; ++kb) {
+            tc::mbar_wait(&full_bar[stage], phase);
+            tc::wgmma_fence();
+            const uint64_t ad = a_desc0 + (uint64_t)(stage * (kAStageBytes >> 4));
+            const uint64_t bd = b_desc0 + (uint64_t)(stage * (p.b_bytes >> 4));
 #pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        __stcg(wslice + ((c >> 2) + i) * kBlockM, make_uint4(r[4 * i], r[4 * i + 1], r[4 * i + 2], r[4 * i + 3]));
-                }
-                tc::tc_fence_before();
+            for (int k = 0; k < kBlockK / 16; ++k) {
+#pragma unroll
+                for (int j = 0; j < kNJ; ++j)   // chunk j: B rows [32 j, 32 j + 32) = +4096 bytes
+                    tc::wgmma_m64n32k16(acc[j], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k + 256 * j));
+            }
+            tc::wgmma_commit();
+            tc::wgmma_wait<1>();              // the previous k-block's MMAs have finished reading their slot
+            if (prev >= 0) {
                 __syncwarp();
-                if (lane == 0) {
-                    if constexpr (kPair) tc::mbar_arrive_cluster(&tempty_bar[acc], 0); else tc::mbar_arrive(&tempty_bar[acc]);
-                }
-                __threadfence();
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (threadIdx.x == 64) {
-                    unsigned int* tk = p.ws_ticket + (nt * tiles_mp + mt);
-                    const unsigned int t = atomicAdd(tk, 1u);
-                    const bool last = (t == (unsigned int)(p.ksplit - 1));
-                    if (last) *tk = 0u;                     // ready for the next launch (stream order)
-                    s_flag[0] = last ? 1 : 0;
-                }
-                asm volatile("bar.sync 1, 256;" ::: "memory");
-                run_epilogue = s_flag[0] != 0;
-                reduce = true;
-                __threadfence();
+                if (lane == 0) tc::mbar_arrive(&empty_bar[prev]);
             }
+            prev = stage;
+            if (++stage == S) { stage = 0; phase ^= 1u; }
+        }
+        tc::wgmma_wait<0>();
+    }
+    // every MMA of both warpgroups has retired: the operand ring becomes the accumulator staging tile
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    {
+        const int r0 = wg * 64 + warp * 16 + (lane >> 2);
+#pragma unroll
+        for (int j = 0; j < kNJ; ++j)
+#pragma unroll
+            for (int i = 0; i < 16; i += 2) {
+                const int r = r0 + 8 * ((i >> 1) & 1);
+                const int c = j * 32 + 8 * (i >> 2) + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(stg + r * kLds + c) = make_float2(acc[j][i], acc[j][i + 1]);
+            }
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
 
-            if (!run_epilogue) {
-                // another slice finishes this tile
-            } else if (TC_DEBUG_MODE() & 2) {
-                // (profiling) accumulator is dropped: measures mainloop + handshake only
-            } else if constexpr (kEpi != 2) {
-                // ---- TMEM -> registers -> swizzled smem box -> one TMA store per 32-column chunk.  Per-thread 16-byte
-                // global stores touch 32 different lines per instruction (LSU: 16 B/clk instead of 128 B/clk) and cost
-                // 30-35 % of the K = 320 launches (scripts/prof_epilogue.py, mode 0 vs 1).  The arithmetic runs on
-                // packed fp32 pairs (FFMA2 / FADD2 / FMUL2): the epilogue is instruction-issue bound at K = 320, and the
-                // staging box is double-buffered so a chunk never waits for the previous chunk's TMA store to drain
-                // (the in-kernel timeline showed ~1400 cycles per chunk, mostly that wait).
-                const int half_bn = BN >> 1;
-                const __half* b2row =
-                    p.bias2 ? p.bias2 + (long long)(row_ok ? fdiv((int)m, p.fd_b2) : 0) * p.bias2_ld + (long long)nt * BN : nullptr;
-                const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = tn * p.TN;
-                const int dbg = TC_DEBUG_MODE();
-                const tc::f32x2 rstd2 = tc::pk2(ln_rstd, ln_rstd), rm2 = tc::pk2(ln_rm, ln_rm);
-                const tc::f32x2 scale2 = tc::pk2(p.acc_scale, p.acc_scale);
-                uint32_t r[32];
-                uint32_t gr[4][16];                                    // GEGLU: {value, gate} x two 16-column halves of a chunk
-                tc::f32x2 rs_sum2 = 0ull, rs_sq2 = 0ull;
-                if (kEpi == 0 && !reduce && cg * 32 < width) tc::tmem_ld32(taddr + (uint32_t)(cg * 32), r);
-#pragma unroll 1
-                for (int jc = 0; jc < 4; ++jc) {
-                    const int c = (cg + 2 * jc) * 32;
-                    if (c >= width) break;
-                    uint32_t pk[16];                                   // the chunk's 32 outputs of this row, fp16 pairs
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(8, ti) }
-                    if constexpr (kEpi == 0) {
-                        // register-path residual (scaled accumulators only; otherwise it rides the tensor core)
-                        uint4 rr[4];
-                        if (rrow) {
+    if (p.ksplit > 1) {
+        // park this slice, take a ticket; only the last slice of the tile goes on and sums the slices in slice order
+        float* ws_tile = p.ws_partial + (long long)tile * p.ksplit * kBlockM * kBNp;
+        float4* wslice = reinterpret_cast<float4*>(ws_tile + (long long)ks * kBlockM * kBNp);
+        for (int i = et; i < kBlockM * kBNp / 4; i += kEpiThreads) {
+            const int r = i / (kBNp / 4), c4 = i - r * (kBNp / 4);
+            __stcg(wslice + i, *reinterpret_cast<const float4*>(stg + r * kLds + 4 * c4));
+        }
+        __threadfence();
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (et == 0) {
+            unsigned int* tk = p.ws_ticket + tile;
+            const unsigned int t = atomicAdd(tk, 1u);
+            const bool last = (t == (unsigned int)(p.ksplit - 1));
+            if (last) *tk = 0u;                     // ready for the next launch (stream order)
+            s_flag[0] = last ? 1 : 0;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (s_flag[0] == 0) return;
+        __threadfence();
+        for (int i = et; i < kBlockM * kBNp / 4; i += kEpiThreads) {
+            const int r = i / (kBNp / 4), c4 = i - r * (kBNp / 4);
+            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int sl = 0; sl < p.ksplit; ++sl) {
+                const float4 u = __ldcg(reinterpret_cast<const float4*>(ws_tile + (long long)sl * kBlockM * kBNp) + i);
+                s.x += u.x; s.y += u.y; s.z += u.z; s.w += u.w;
+            }
+            *reinterpret_cast<float4*>(stg + r * kLds + 4 * c4) = s;
+        }
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+    }
+
+    // ---------------------------------------------------------------------- epilogue: one row per thread, 2 column groups
+    const int row = et & 127;
+    const int cg = et >> 7;
+    const int rx = row % p.TW;
+    const int ry = (row / p.TW) % p.TH;
+    const int rn = row / (p.TW * p.TH);
+    const int x = tx * p.TW + rx, y = ty * p.TH + ry, n = tn * p.TN + rn;
+    const bool row_ok = (rn < p.TN) && (x < p.oW) && (y < p.oH) && (n < p.oN);
+    const long long m = ((long long)n * p.oH + y) * p.oW + x;
+    const bool geglu = p.geglu != 0;
+    const int width = geglu ? (BN >> 1) : BN;                   // output columns per tile
+    const int split = ((width / 16 + 1) / 2) * 16;              // group 0: [0, split), group 1: [split, width)
+    const int c_begin = cg == 0 ? 0 : split;
+    const int c_end = cg == 0 ? split : width;
+    const int out_cols = geglu ? (p.n_cols >> 1) : p.n_cols;
+    const int col0 = nt * width;                                // first output column of the tile
+
+    float mean = 0.f, rstd = 1.f;
+    if (p.ln_stats && row_ok) {
+        if (p.ln_nslots > 0) {
+            // partial {sum, sumsq} slots written by the producer GEMM's epilogue (fixed order: deterministic)
+            float s1 = 0.f, s2 = 0.f;
+            const float2* ps = p.ln_stats + m * p.ln_nslots;
+            for (int i = 0; i < p.ln_nslots; ++i) {
+                const float2 st = __ldg(ps + i);
+                s1 += st.x;
+                s2 += st.y;
+            }
+            mean = s1 * p.ln_inv_c;
+            rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
+        } else {
+            const float2 st = __ldg(p.ln_stats + m);
+            mean = st.x;
+            rstd = st.y;
+        }
+    }
+    const float* srow = stg + row * kLds;
+    const __half* b2row = (p.bias2 && row_ok) ? p.bias2 + (m / p.bias2_rows_per) * p.bias2_ld + (long long)nt * BN : nullptr;
+    const __half* rrow = (p.res && row_ok) ? p.res + m * p.ldr + (long long)nt * BN : nullptr;
+    __half* orow = p.out + m * p.ldc + col0;
+    float rs_sum = 0.f, rs_sq = 0.f;
+    if (row_ok) {
+        for (int c = c_begin; c < c_end; c += 8) {
+            const int nvalid = min(8, out_cols - (col0 + c));
+            if (nvalid <= 0) break;
+            float v[8];
+            if (!geglu) {
 #pragma unroll
-                            for (int hh = 0; hh < 4; ++hh) rr[hh] = *reinterpret_cast<const uint4*>(rrow + c + hh * 8);
-                        }
-                        tc::f32x2 v[16];
-                        if (!reduce) {
-                            tc::tmem_ld_wait();
+                for (int i = 0; i < 8; ++i) v[i] = rstd * (srow[c + i] - mean * s_u[c + i]) + s_bias[c + i];
+                if (b2row) {
+                    if (nvalid == 8) {
+                        const uint4 u = __ldg(reinterpret_cast<const uint4*>(b2row + c));
+                        const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = tc::pk2u(r[2 * i], r[2 * i + 1]);
-                            // next chunk's accumulator read flies while this one is finished, staged and stored
-                            if (c + 64 < width) tc::tmem_ld32(taddr + (uint32_t)(c + 64), r);
-                        } else {
-                            // split-K: sum the parked slices in slice order (L2 reads: other SMs wrote them)
-                            const uint4* wsrc = reinterpret_cast<const uint4*>(p.ws_partial + (long long)(nt * tiles_mp + mt) * p.ksplit * kBlockM * BN) +
-                                                (c >> 2) * kBlockM + row;
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = 0ull;
-                            for (int sl = 0; sl < p.ksplit; ++sl) {
-                                const uint4* src4 = wsrc + (long long)sl * (kBlockM * BN / 4);
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) {
-                                    const uint4 u = __ldcg(src4 + i * kBlockM);
-                                    v[2 * i] = tc::add2(v[2 * i], tc::pk2u(u.x, u.y));
-                                    v[2 * i + 1] = tc::add2(v[2 * i + 1], tc::pk2u(u.z, u.w));
-                                }
-                            }
-                        }
-                        // rstd*(acc - mean*u) + bias  ==  rstd*acc + (rm*u + bias), rm = -rstd*mean: two packed FMAs per pair
-                        // (rstd = 1, rm = 0, u = 0 without a folded LayerNorm: exactly acc + bias).  The per-column vectors
-                        // are read with 32-bit shared addresses: through generic pointers every read cost six 64-bit
-                        // address instructions (profiles/r02_ncu_gemm_geglu_insitu.txt).
-                        {
-                            const uint32_t ab = sbias_a + (uint32_t)c * 4u, au = ab + 1024u;
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                float4 u4, b4;
-                                tc::lds128(au + 16u * i, u4);
-                                tc::lds128(ab + 16u * i, b4);
-                                v[2 * i] = tc::fma2(rstd2, v[2 * i], tc::fma2(rm2, tc::pk2(u4.x, u4.y), tc::pk2(b4.x, b4.y)));
-                                v[2 * i + 1] = tc::fma2(rstd2, v[2 * i + 1], tc::fma2(rm2, tc::pk2(u4.z, u4.w), tc::pk2(b4.z, b4.w)));
-                            }
-                        }
-                        if (b2row) {
-#pragma unroll
-                            for (int hh = 0; hh < 4; ++hh) {
-                                const uint4 u = __ldg(reinterpret_cast<const uint4*>(b2row + c) + hh);
-                                v[4 * hh] = tc::add2(v[4 * hh], tc::f2_from_h2(u.x));
-                                v[4 * hh + 1] = tc::add2(v[4 * hh + 1], tc::f2_from_h2(u.y));
-                                v[4 * hh + 2] = tc::add2(v[4 * hh + 2], tc::f2_from_h2(u.z));
-                                v[4 * hh + 3] = tc::add2(v[4 * hh + 3], tc::f2_from_h2(u.w));
-                            }
-                        }
-                        if (p.acc_scale != 1.0f) {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] = tc::mul2(v[i], scale2);
-                        }
-                        if (rrow) {
-#pragma unroll
-                            for (int hh = 0; hh < 4; ++hh) {
-                                v[4 * hh] = tc::add2(v[4 * hh], tc::f2_from_h2(rr[hh].x));
-                                v[4 * hh + 1] = tc::add2(v[4 * hh + 1], tc::f2_from_h2(rr[hh].y));
-                                v[4 * hh + 2] = tc::add2(v[4 * hh + 2], tc::f2_from_h2(rr[hh].z));
-                                v[4 * hh + 3] = tc::add2(v[4 * hh + 3], tc::f2_from_h2(rr[hh].w));
-                            }
-                        }
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) pk[i] = tc::h2_from_f2(v[i]);
-                        if (p.row_stats) {
-                            // statistics of the values the consumer will read: the fp16-rounded outputs
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) {
-                                const tc::f32x2 f = tc::f2_from_h2(pk[i]);
-                                rs_sum2 = tc::add2(rs_sum2, f);
-                                rs_sq2 = tc::fma2(f, f, rs_sq2);
-                            }
+                        for (int i = 0; i < 4; ++i) {
+                            const float2 f = __half22float2(h2[i]);
+                            v[2 * i] += f.x;
+                            v[2 * i + 1] += f.y;
                         }
                     } else {
-                        // weight rows of this N tile are [value half (BN/2) | gate half (BN/2)].  All four 16-column TMEM
-                        // reads of a chunk are in flight at once, and the NEXT chunk's reads are issued right after this
-                        // chunk's arithmetic, so their latency (~200 cycles each) hides behind the staging / TMA store.
-                        if (jc == 0) {
-                            tc::tmem_ld16(taddr + (uint32_t)c, gr[0]);
-                            tc::tmem_ld16(taddr + (uint32_t)(half_bn + c), gr[1]);
-                            tc::tmem_ld16(taddr + (uint32_t)(c + 16), gr[2]);
-                            tc::tmem_ld16(taddr + (uint32_t)(half_bn + c + 16), gr[3]);
-                        }
-                        tc::tmem_ld_wait();
-                        if (threadIdx.x == 64 && jc == 0) { TC_TRACE(14, ti) }   // TMEM reads landed
-#pragma unroll
-                        for (int h16 = 0; h16 < 2; ++h16) {
-                            const uint32_t (&ra)[16] = gr[2 * h16];
-                            const uint32_t (&rg)[16] = gr[2 * h16 + 1];
-                            const int cc = c + h16 * 16;
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const uint32_t aa = sbias_a + (uint32_t)cc * 4u + 16u * i, ag = aa + (uint32_t)half_bn * 4u;
-                                float4 ba, bg, ua, ug;
-                                tc::lds128(aa, ba);
-                                tc::lds128(ag, bg);
-                                tc::lds128(aa + 1024u, ua);
-                                tc::lds128(ag + 1024u, ug);
-                                tc::f32x2 a01 = tc::pk2u(ra[4 * i], ra[4 * i + 1]), a23 = tc::pk2u(ra[4 * i + 2], ra[4 * i + 3]);
-                                tc::f32x2 g01 = tc::pk2u(rg[4 * i], rg[4 * i + 1]), g23 = tc::pk2u(rg[4 * i + 2], rg[4 * i + 3]);
-                                a01 = tc::fma2(rstd2, a01, tc::fma2(rm2, tc::pk2(ua.x, ua.y), tc::pk2(ba.x, ba.y)));
-                                a23 = tc::fma2(rstd2, a23, tc::fma2(rm2, tc::pk2(ua.z, ua.w), tc::pk2(ba.z, ba.w)));
-                                g01 = tc::fma2(rstd2, g01, tc::fma2(rm2, tc::pk2(ug.x, ug.y), tc::pk2(bg.x, bg.y)));
-                                g23 = tc::fma2(rstd2, g23, tc::fma2(rm2, tc::pk2(ug.z, ug.w), tc::pk2(bg.z, bg.w)));
-                                pk[h16 * 8 + 2 * i] = tc::h2_from_f2(tc::geglu_mul2(a01, g01));
-                                pk[h16 * 8 + 2 * i + 1] = tc::h2_from_f2(tc::geglu_mul2(a23, g23));
-                            }
-                        }
-                        {
-                            const int cn = c + 64;                       // this column group's next chunk
-                            if (cn < width) {
-                                tc::tmem_ld16(taddr + (uint32_t)cn, gr[0]);
-                                tc::tmem_ld16(taddr + (uint32_t)(half_bn + cn), gr[1]);
-                                tc::tmem_ld16(taddr + (uint32_t)(cn + 16), gr[2]);
-                                tc::tmem_ld16(taddr + (uint32_t)(half_bn + cn + 16), gr[3]);
-                            }
-                        }
+                        for (int i = 0; i < nvalid; ++i) v[i] += __half2float(b2row[c + i]);
                     }
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(9, ti) }      // math done
-                    if (p.batch_store) {
-                        // ---- short-K launches (epilogue-bound): every chunk of the tile has its own staging box, so the box-free
-                        // wait, the proxy fence, the barrier and the store issue — ~1000 cycles of serial latency per chunk in the
-                        // in-kernel timeline (profiles/r02_gemm_trace_k320.txt) — are paid once per tile, after the chunk loop
-                        if (jc == 0) {
-                            if (store_warp) {
-                                if (tc::elect_one()) tc::bulk_wait_group_read<0>();     // the previous tile's stores have read every box
-                            }
-                            if (warp_box) __syncwarp();
-                            else if (cg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-                            else asm volatile("bar.sync 3, 128;" ::: "memory");
-                            if (threadIdx.x == 64) { TC_TRACE(10, ti) }     // staging boxes free
-                        }
-                        const uint32_t stg_row_b = stg_row + (uint32_t)jc * 16384u;
-                        if (!(dbg & 16))
-#pragma unroll
-                        for (int hh = 0; hh < 4; ++hh) {
-                            const uint32_t dst = stg_row_b + ((((uint32_t)hh) ^ stg_swz) << 4);
-                            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[4 * hh]),
-                                         "r"(pk[4 * hh + 1]), "r"(pk[4 * hh + 2]), "r"(pk[4 * hh + 3])
-                                         : "memory");
-                        }
-                        if (threadIdx.x == 64 && jc == 0) { TC_TRACE(11, ti) }     // staged
-                        continue;
-                    }
-                    // two staging boxes in rotation: only the store issued two chunks ago must have drained this one
-                    const uint32_t buf = n_stores & (uint32_t)(p.stage_bufs - 1);
-                    uint8_t* stg_b = stg + buf * 16384u;
-                    const uint32_t stg_row_b = stg_row + buf * 16384u;
-                    ++n_stores;
-                    if (store_warp) {
-                        if (tc::elect_one()) {
-                            if (p.stage_bufs == 2) tc::bulk_wait_group_read<1>(); else tc::bulk_wait_group_read<0>();
-                        }
-                    }
-                    if (warp_box) __syncwarp();
-                    else if (cg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-                    else asm volatile("bar.sync 3, 128;" ::: "memory");
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(10, ti) }     // staging box free
-                    if (!(dbg & 16))
-#pragma unroll
-                    for (int hh = 0; hh < 4; ++hh) {
-                        const uint32_t dst = stg_row_b + ((((uint32_t)hh) ^ stg_swz) << 4);
-                        asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(dst), "r"(pk[4 * hh]),
-                                     "r"(pk[4 * hh + 1]), "r"(pk[4 * hh + 2]), "r"(pk[4 * hh + 3])
-                                     : "memory");
-                    }
-                    if (!(dbg & 8)) tc::fence_proxy_async_smem();
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(11, ti) }     // staged + fenced
-                    if (warp_box) __syncwarp();
-                    else if (cg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-                    else asm volatile("bar.sync 3, 128;" ::: "memory");
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(12, ti) }
-                    if (store_warp && !(dbg & 1)) {
-                        if (warp_box) {
-                            if (warp_rows_in_tile) {
-                                if (tc::elect_one()) {
-                                    tc::tma_store_4d(stg_b, &p.tmOw, nt * width + c, x0 + wx, y0 + wy, n0 + wn);
-                                    tc::bulk_commit_group();
-                                }
-                            }
-                        } else if (tc::elect_one()) {
-                            tc::tma_store_4d(stg_b, &p.tmO, nt * width + c, x0, y0, n0);
-                            tc::bulk_commit_group();
-                        }
-                    }
-                    if (threadIdx.x == 64 && jc == 0) { TC_TRACE(13, ti) }     // store issued
                 }
-                if (p.batch_store) {
-                    // one proxy fence, one barrier, then the whole tile's stores from one elected lane and ONE commit
-                    if (!(dbg & 8)) tc::fence_proxy_async_smem();
-                    if (warp_box) __syncwarp();
-                    else if (cg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-                    else asm volatile("bar.sync 3, 128;" ::: "memory");
-                    if (threadIdx.x == 64) { TC_TRACE(12, ti) }
-                    if (store_warp && !(dbg & 1) && (!warp_box || warp_rows_in_tile)) {
-                        if (tc::elect_one()) {
-                            for (int jc = 0; jc < 4; ++jc) {
-                                const int c = (cg + 2 * jc) * 32;
-                                if (c >= width) break;
-                                if (warp_box) tc::tma_store_4d(stg + jc * 16384, &p.tmOw, nt * width + c, x0 + wx, y0 + wy, n0 + wn);
-                                else tc::tma_store_4d(stg + jc * 16384, &p.tmO, nt * width + c, x0, y0, n0);
-                            }
-                            tc::bulk_commit_group();
+                if (p.acc_scale != 1.0f) {
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) v[i] *= p.acc_scale;
+                }
+                if (rrow) {
+                    if (nvalid == 8) {
+                        const uint4 u = *reinterpret_cast<const uint4*>(rrow + c);
+                        const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const float2 f = __half22float2(h2[i]);
+                            v[2 * i] += f.x;
+                            v[2 * i + 1] += f.y;
                         }
-                    }
-                    if (threadIdx.x == 64) { TC_TRACE(13, ti) }     // stores issued
-                }
-                float rs_sum = 0.f, rs_sq = 0.f;
-                if (kEpi == 0 && p.row_stats) {
-                    float s0, s1, q0, q1;
-                    tc::unpk2(rs_sum2, s0, s1);
-                    tc::unpk2(rs_sq2, q0, q1);
-                    rs_sum = s0 + s1;
-                    rs_sq = q0 + q1;
-                }
-                if (kEpi == 0 && p.row_stats) {
-                    // one slot per N tile: group 1 hands {sum, sumsq} of its columns to the warp of group 0 that owns
-                    // the same rows (64-thread named barrier, group 1 only arrives).  Group 1 may run one tile ahead of
-                    // group 0 (two TMEM accumulators), so buffers AND barrier ids alternate with the tile parity: two
-                    // arrivals of the same warp on one id would complete the barrier without group 0.
-                    float2* hand = s_rs + (ti & 1) * 128 + row;
-                    const int bar_id = 4 + q + 4 * (ti & 1);
-                    if (cg == 1) {
-                        *hand = make_float2(rs_sum, rs_sq);
-                        asm volatile("bar.arrive %0, 64;" ::"r"(bar_id) : "memory");
                     } else {
-                        asm volatile("bar.sync %0, 64;" ::"r"(bar_id) : "memory");
-                        const float2 o = *hand;
-                        if (row_ok) p.row_stats[m * p.row_stats_slots + nt] = make_float2(rs_sum + o.x, rs_sq + o.y);
-                    }
-                }
-            } else if (!geglu) {
-                __half* orow = p.out + m * p.ldc + (long long)nt * BN;
-                const __half* b2row =
-                    p.bias2 ? p.bias2 + (long long)(row_ok ? fdiv((int)m, p.fd_b2) : 0) * p.bias2_ld + (long long)nt * BN : nullptr;
-                const float* brow = p.bias ? p.bias + (long long)nt * BN : nullptr;
-#pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int c = c_begin + j * 16;
-                    if (c >= c_end) break;
-                    uint32_t r[16];
-                    tc::tmem_ld16(taddr + (uint32_t)c, r);
-                    tc::tmem_ld_wait();
-                    const int nvalid = p.n_cols - (nt * BN + c);
-                    if (!row_ok || nvalid <= 0) continue;
-                    float v[16];
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-                    if (vec_ok) {
-                        if (p.ln_u) {
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float4 u4 = reinterpret_cast<const float4*>(su + c)[i];
-                                v[4 * i] = ln_rstd * (v[4 * i] - ln_mean * u4.x);
-                                v[4 * i + 1] = ln_rstd * (v[4 * i + 1] - ln_mean * u4.y);
-                                v[4 * i + 2] = ln_rstd * (v[4 * i + 2] - ln_mean * u4.z);
-                                v[4 * i + 3] = ln_rstd * (v[4 * i + 3] - ln_mean * u4.w);
-                            }
-                        }
-                        if (brow) {
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float4 b4 = reinterpret_cast<const float4*>(sbias + c)[i];
-                                v[4 * i] += b4.x;
-                                v[4 * i + 1] += b4.y;
-                                v[4 * i + 2] += b4.z;
-                                v[4 * i + 3] += b4.w;
-                            }
-                        }
-                        if (b2row) {
-#pragma unroll
-                            for (int hh = 0; hh < 2; ++hh) {
-                                const uint4 u = __ldg(reinterpret_cast<const uint4*>(b2row + c) + hh);
-                                const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) {
-                                    const float2 f = __half22float2(h2[i]);
-                                    v[hh * 8 + 2 * i] += f.x;
-                                    v[hh * 8 + 2 * i + 1] += f.y;
-                                }
-                            }
-                        }
-                        if (p.acc_scale != 1.0f) {
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) v[i] *= p.acc_scale;
-                        }
-                        if (rrow) {
-#pragma unroll
-                            for (int hh = 0; hh < 2; ++hh) {
-                                const __half2* h2 = reinterpret_cast<const __half2*>(&rres[2 * j + hh]);
-#pragma unroll
-                                for (int i = 0; i < 4; ++i) {
-                                    const float2 f = __half22float2(h2[i]);
-                                    v[hh * 8 + 2 * i] += f.x;
-                                    v[hh * 8 + 2 * i + 1] += f.y;
-                                }
-                            }
-                        }
-                        store_row16(orow + c, v, 16);
-                    } else {
-                        // generic path for narrow outputs (n_cols = 3, 4, 8 ...): scalar loads / stores
-#pragma unroll
-                        for (int i = 0; i < 16; ++i) {
-                            if (i < nvalid) {
-                                if (brow) v[i] += brow[c + i];
-                                if (b2row) v[i] += __half2float(b2row[c + i]);
-                                v[i] *= p.acc_scale;
-                                if (rrow) v[i] += __half2float(rrow[c + i]);
-                            }
-                        }
-                        store_row16(orow + c, v, nvalid);
+                        for (int i = 0; i < nvalid; ++i) v[i] += __half2float(rrow[c + i]);
                     }
                 }
             } else {
-                // weight rows of this N tile are [value half (BN/2) | gate half (BN/2)]; output tile is BN/2 wide
-                const int half_bn = BN >> 1;
-                __half* orow = p.out + m * p.ldc + (long long)nt * half_bn;
-                const float* brow = p.bias ? p.bias + (long long)nt * BN : nullptr;
+                // weight rows of this N tile are [value half (BN/2) | gate half (BN/2)]
+                const int g = c + width;
 #pragma unroll
-                for (int j = 0; j < 8; ++j) {
-                    const int c = c_begin + j * 16;
-                    if (c >= c_end) break;
-                    uint32_t ra[16], rg[16];
-                    tc::tmem_ld16(taddr + (uint32_t)c, ra);
-                    tc::tmem_ld16(taddr + (uint32_t)(half_bn + c), rg);
-                    tc::tmem_ld_wait();
-                    if (!row_ok) continue;
-                    float v[16];
-                    const float* urow = p.ln_u ? p.ln_u + (long long)nt * BN : nullptr;
+                for (int i = 0; i < 8; ++i) {
+                    const float a = rstd * (srow[c + i] - mean * s_u[c + i]) + s_bias[c + i];
+                    const float xg = rstd * (srow[g + i] - mean * s_u[g + i]) + s_bias[g + i];
+                    v[i] = a * tc::gelu_erf_f(xg);
+                }
+            }
+            if (nvalid == 8) {
+                uint4 u;
+                u.x = pack_h2(v[0], v[1]);
+                u.y = pack_h2(v[2], v[3]);
+                u.z = pack_h2(v[4], v[5]);
+                u.w = pack_h2(v[6], v[7]);
+                *reinterpret_cast<uint4*>(orow + c) = u;
+                if (p.row_stats) {
+                    // statistics of the values the consumer will read: the fp16-rounded outputs
+                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
                     for (int i = 0; i < 4; ++i) {
-                        float4 ba = make_float4(0.f, 0.f, 0.f, 0.f), bg = ba;
-                        if (brow) {
-                            ba = reinterpret_cast<const float4*>(sbias + c)[i];
-                            bg = reinterpret_cast<const float4*>(sbias + half_bn + c)[i];
-                        }
-                        float a0 = __uint_as_float(ra[4 * i]), a1 = __uint_as_float(ra[4 * i + 1]);
-                        float a2 = __uint_as_float(ra[4 * i + 2]), a3 = __uint_as_float(ra[4 * i + 3]);
-                        float g0 = __uint_as_float(rg[4 * i]), g1 = __uint_as_float(rg[4 * i + 1]);
-                        float g2 = __uint_as_float(rg[4 * i + 2]), g3 = __uint_as_float(rg[4 * i + 3]);
-                        if (urow) {
-                            const float4 ua = reinterpret_cast<const float4*>(su + c)[i];
-                            const float4 ug = reinterpret_cast<const float4*>(su + half_bn + c)[i];
-                            a0 = ln_rstd * (a0 - ln_mean * ua.x);
-                            a1 = ln_rstd * (a1 - ln_mean * ua.y);
-                            a2 = ln_rstd * (a2 - ln_mean * ua.z);
-                            a3 = ln_rstd * (a3 - ln_mean * ua.w);
-                            g0 = ln_rstd * (g0 - ln_mean * ug.x);
-                            g1 = ln_rstd * (g1 - ln_mean * ug.y);
-                            g2 = ln_rstd * (g2 - ln_mean * ug.z);
-                            g3 = ln_rstd * (g3 - ln_mean * ug.w);
-                        }
-                        v[4 * i] = (a0 + ba.x) * tc::gelu_erf_f(g0 + bg.x);
-                        v[4 * i + 1] = (a1 + ba.y) * tc::gelu_erf_f(g1 + bg.y);
-                        v[4 * i + 2] = (a2 + ba.z) * tc::gelu_erf_f(g2 + bg.z);
-                        v[4 * i + 3] = (a3 + ba.w) * tc::gelu_erf_f(g3 + bg.w);
+                        const float2 f = __half22float2(h2[i]);
+                        rs_sum += f.x + f.y;
+                        rs_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, rs_sq));
                     }
-                    store_row16(orow + c, v, 16);
+                }
+            } else {
+                for (int i = 0; i < nvalid; ++i) {
+                    const __half h = __float2half_rn(v[i]);
+                    orow[c + i] = h;
+                    const float f = __half2float(h);
+                    rs_sum += f;
+                    rs_sq = fmaf(f, f, rs_sq);
                 }
             }
-            if (!(kEpi == 0 && p.ksplit > 1)) {      // (split-K released the accumulator right after parking it)
-                tc::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) {
-                    if constexpr (kPair) tc::mbar_arrive_cluster(&tempty_bar[acc], 0); else tc::mbar_arrive(&tempty_bar[acc]);
-                }
-            }
-            if (threadIdx.x == 64) { TC_TRACE(7, ti) }
-            acc ^= 1;
-            if (acc == 0) acc_phase ^= 1u;
         }
     }
-#undef TC_DECODE_TILE
-#undef TC_TILE_NT
-
-    if (p.tma_store && warp >= 2) {
-        if (tc::elect_one()) tc::bulk_wait_group<0>();      // the lane that committed the store groups
-    }
-    tc::tc_fence_before();
-    if constexpr (kPair) tc::cluster_sync_all(); else __syncthreads();   // the peer may still read our smem / barriers
-    if (warp == 2) {
-        tc::tc_fence_after();
-        if constexpr (kPair) tc::tmem_dealloc_pair(tmem_base, kTmemCols); else tc::tmem_dealloc(tmem_base, kTmemCols);
+    if (p.row_stats) {
+        // one slot per N tile: column group 1 hands its partials to the thread of group 0 that owns the same row
+        if (cg == 1) s_rs[row] = make_float2(rs_sum, rs_sq);
+        asm volatile("bar.sync 1, 256;" ::: "memory");
+        if (cg == 0 && row_ok) {
+            const float2 o = s_rs[row];
+            p.row_stats[m * p.row_stats_slots + nt] = make_float2(rs_sum + o.x, rs_sq + o.y);
+        }
     }
 }
 
-// Tile-shape heuristic: pick (block_n, single / CTA-pair) minimising   waves x per-tile cycles   with a small model
-// measured on B200 (tensor rate vs. TMA ingest per k-block, see below), plus ~1500 cycles of per-tile pipeline fill /
-// epilogue tail.  Matters for the 10x16 and 5x8 UNet levels (M = 5120 / 1280 rows), where
-// one wave of 256-wide tiles leaves most SMs idle.
+// Tile-shape heuristic: pick (block_n, k-slices) minimising   waves x per-tile cycles   with a small model of one
+// k-block (M128 x bn x K64): tensor time at the data-sheet dense fp16 rate (989 TFLOP/s over 132 SMs: ~4 bn cycles), or
+// the ingest of its operands (A 16 KB + B bn x 128 B) at an assumed 52 B/clk/SM from L2, plus an assumed ~1500 cycles of
+// per-tile pipeline fill / epilogue tail.  The ingest rate, the per-tile overhead and the split-K overhead below are model
+// parameters, not measured on the H100.  Matters for
+// the 10x16 and 5x8 UNet levels (M = 5120 / 1280 rows), where one wave of 256-wide tiles leaves most SMs idle.
 struct TileChoice {
     int bn;
-    bool pair;
     int ksplit;
 };
 
-// max_ksplit > 1: the launch may split its K loop (plain TMA-store epilogue, workspace available)
 TileChoice choose_tiles(int tiles_m, int n_cols, int kblocks, int forced_bn, int sms, int max_ksplit, long long ws_floats) {
     const int n16 = (n_cols + 15) / 16 * 16;
-    TileChoice best{n16 <= 256 ? n16 : 256, false, 1};
+    TileChoice best{n16 <= 256 ? n16 : 256, 1};
     double best_cost = 1e30;
     for (int bn = 256; bn >= 16; bn -= 16) {
         if (forced_bn > 0 && bn != forced_bn) continue;
         if (forced_bn == 0) {
             if (bn > n16) continue;
-            // whole tiles only; 32-column granularity keeps the TMA-store epilogue applicable
             if (n16 > 256 ? (n16 % bn != 0 || bn < 64 || bn % 32 != 0) : (bn != n16)) continue;
         }
+        const int bnp = (bn + 31) / 32 * 32;
         const int tiles_n = (n_cols + bn - 1) / bn;
-        for (int pair = 0; pair < 2; ++pair) {
-            if (pair && tiles_m < 2) continue;
-            // one k-block (M128 x bn x K64 per CTA): tensor time ~2.5 bn cycles at the sustained rate, or the TMA ingest
-            // of its operands at the ~52 B/clk/SM the L2 delivers (A 16 KB + B bn x 128 B, halved by a pair) — measured
-            // with scripts/sweep_tiles.py: e.g. conv 640->640 @20x32 runs 148 us with bn 128 and 126 us with bn 160
-            const double tensor = 2.5 * bn;
-            const double ingest = (16384.0 + (double)bn * (pair ? 64.0 : 128.0)) / 52.0;
-            double kb_cycles = tensor > ingest ? tensor : ingest;
-            if (kb_cycles < 200.0) kb_cycles = 200.0;
-            const long long tiles = pair ? (long long)((tiles_m + 1) / 2) * tiles_n : (long long)tiles_m * tiles_n;
-            const int slots = pair ? sms / 2 : sms;
-            for (int ks = 1; ks <= max_ksplit; ++ks) {
-                const int kb_per = (kblocks + ks - 1) / ks;
-                if (ks > 1) {
-                    // slices of >= 8 k-blocks, whole-tile workspace, and the bn must leave the TMA-store path applicable
-                    if (kb_per < 8 || (kb_per * (ks - 1)) >= kblocks) continue;
-                    const long long tiles_all = (long long)(pair ? 2 * ((tiles_m + 1) / 2) : tiles_m) * tiles_n;
-                    if (tiles_all * ks * 128 * bn > ws_floats || tiles_all * 4 > TC_GEMM_WS_TICKET_BYTES) continue;
-                    if (bn % 32 != 0 || n_cols % bn != 0) continue;
-                }
-                // split-K overhead, paid once in the launch's tail (earlier waves park under the next item's main loop): every
-                // slice parks 128 x bn floats in L2, a fence + ticket round trip, and the last slice reads ks of them back
-                // before the usual epilogue.  Measured (scripts/ksplit_ab.py, bn 256, 2 slices): ~10 us = ~20k cycles over
-                // the unsplit launch at equal k-blocks per CTA; a 5 % margin keeps marginal cases unsplit.
-                const double red = ks > 1 ? 22000.0 * (bn / 256.0) * (0.5 + 0.25 * ks) : 0.0;
-                const double tile_cost = (double)kb_per * kb_cycles + 1500.0 + 4.0 * bn;
-                const long long waves = (tiles * ks + slots - 1) / slots;
-                const double cost = ((double)waves * tile_cost + red) * (ks > 1 ? 1.05 : 1.0);
-                if (cost < best_cost) {
-                    best_cost = cost;
-                    best = TileChoice{bn, pair != 0, ks};
-                }
+        const double tensor = 4.0 * bnp;
+        const double ingest = (16384.0 + (double)bnp * 128.0) / 52.0;
+        double kb_cycles = tensor > ingest ? tensor : ingest;
+        if (kb_cycles < 200.0) kb_cycles = 200.0;
+        const long long tiles = (long long)tiles_m * tiles_n;
+        for (int ks = 1; ks <= max_ksplit; ++ks) {
+            const int kb_per = (kblocks + ks - 1) / ks;
+            if (ks > 1) {
+                // slices of >= 8 k-blocks, whole-tile workspace
+                if (kb_per < 8 || (kb_per * (ks - 1)) >= kblocks) continue;
+                if (tiles * ks * 128 * bnp > ws_floats || tiles * 4 > TC_GEMM_WS_TICKET_BYTES) continue;
+                if (bn % 32 != 0 || n_cols % bn != 0) continue;
+            }
+            // split-K overhead (model parameter): every slice parks 128 x bn floats in L2, a fence + ticket round trip, and
+            // the last slice reads ks of them back before the usual epilogue; a 5 % margin keeps marginal cases unsplit
+            const double red = ks > 1 ? 22000.0 * (bn / 256.0) * (0.5 + 0.25 * ks) : 0.0;
+            const double tile_cost = (double)kb_per * kb_cycles + 1500.0 + 4.0 * bn;
+            const long long waves = (tiles * ks + sms - 1) / sms;
+            const double cost = ((double)waves * tile_cost + red) * (ks > 1 ? 1.05 : 1.0);
+            if (cost < best_cost) {
+                best_cost = cost;
+                best = TileChoice{bn, ks};
             }
         }
     }
     return best;
 }
 
+using KernelFn = void (*)(GemmKParams);
+const KernelFn kKernels[8] = {tc_gemm_kernel<1>, tc_gemm_kernel<2>, tc_gemm_kernel<3>, tc_gemm_kernel<4>,
+                              tc_gemm_kernel<5>, tc_gemm_kernel<6>, tc_gemm_kernel<7>, tc_gemm_kernel<8>};
+
 }  // namespace
 
 extern "C" int tc_debug_read_gemm_trace(unsigned long long* host_dst, int count) {
-#if defined(TC_GEMM_TRACE) && TC_GEMM_TRACE
-    if (!host_dst || count <= 0 || count > kTraceCtas * kTraceTiles * kTraceSlots)
-        return tc_host::fail(TC_ERR_INVALID, "tc_debug_read_gemm_trace: bad count");
-    return tc_host::check_cuda(cudaMemcpyFromSymbol(host_dst, g_tc_gemm_trace, (size_t)count * sizeof(unsigned long long)),
-                               "tc_debug_read_gemm_trace");
-#else
     (void)host_dst;
     (void)count;
-    return tc_host::fail(TC_ERR_INVALID, "tc_debug_read_gemm_trace: library built without TC_BUILD_TRACE=1");
-#endif
+    return tc_host::fail(TC_ERR_INVALID, "tc_debug_read_gemm_trace: the GEMM kernel records no timeline");
 }
 
 static int g_last_cfg[4] = {0, 0, 0, 0};
@@ -1134,8 +434,7 @@ extern "C" int tc_debug_last_gemm_config(int* out4) {
 static int g_ksplit_cap = 0;   // profiling: bits 8..11 of the debug mode cap the k-slices of later launches (0 = heuristic)
 extern "C" int tc_debug_set_gemm_mode(int mode) {
     g_ksplit_cap = (mode >> 8) & 15;
-    mode &= 255;
-    return tc_host::check_cuda(cudaMemcpyToSymbol(g_tc_gemm_debug, &mode, sizeof(int)), "tc_debug_set_gemm_mode");
+    return TC_OK;
 }
 
 extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
@@ -1203,11 +502,10 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     p.oN = d->oN;
     p.tiles_x = (d->oW + p.TW - 1) / p.TW;
     p.tiles_y = (d->oH + p.TH - 1) / p.TH;
-    p.tiles_n = (d->oN + p.TN - 1) / p.TN;
-    p.tiles_m = p.tiles_x * p.tiles_y * p.tiles_n;
+    const int tiles_n = (d->oN + p.TN - 1) / p.TN;
+    const long long tiles_m = (long long)p.tiles_x * p.tiles_y * tiles_n;
     TC_CHECK_ARG((long long)d->oN * d->oH * d->oW < (1LL << 31), "tc_conv_gemm: more than 2^31 output rows");
-    static const char* pair_env = getenv("TC_GEMM_PAIR");       // "0" / "1" force (A/B testing), unset = heuristic
-    // split-K only with the plain TMA-store epilogue (no GEGLU, no LayerNorm fold, no row statistics) and a workspace
+    // split-K only for plain epilogues (no GEGLU, no LayerNorm fold, no row statistics) with a workspace
     static const char* ksplit_env = getenv("TC_GEMM_KSPLIT");    // "1" disables, "2".."4" caps (A/B testing)
     int max_ksplit = 4;
     if (ksplit_env && ksplit_env[0] >= '1' && ksplit_env[0] <= '4') max_ksplit = ksplit_env[0] - '0';
@@ -1217,11 +515,12 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     if (geglu || d->ln_stats || d->row_stats || d->n_cols % 16 != 0 || ws_floats == 0 ||
         (reinterpret_cast<uintptr_t>(d->workspace) & 15) != 0)
         max_ksplit = 1;
-    TileChoice choice = choose_tiles(p.tiles_m, d->n_cols, d->taps * (d->a_C / kBlockK), BN, sm_count(), max_ksplit, ws_floats);
+    const int main_kblocks = d->taps * (d->a_C / kBlockK);
+    TileChoice choice = choose_tiles((int)tiles_m, d->n_cols, main_kblocks, BN, sm_count(), max_ksplit, ws_floats);
     BN = choice.bn;
-    bool pair = choice.pair;
-    if (pair_env) pair = (pair_env[0] == '1') && p.tiles_m >= 2;
-    p.ksplit = (pair == choice.pair) ? choice.ksplit : 1;
+    const int BNp = (BN + 31) / 32 * 32;
+    p.ksplit = choice.ksplit;
+    p.kb_per = (main_kblocks + p.ksplit - 1) / p.ksplit;
     p.BN = BN;
     p.tiles_nn = (d->n_cols + BN - 1) / BN;
     p.n_cols = d->n_cols;
@@ -1233,6 +532,7 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     }
     p.kc_per_tap = d->a_C / kBlockK;
     p.a_bytes = (uint32_t)(p.TW * p.TH * p.TN) * 128u;
+    p.b_bytes = (uint32_t)BNp * 128u;
     p.out = reinterpret_cast<__half*>(d->out);
     p.ldc = d->ldc;
     p.bias = d->bias;
@@ -1242,7 +542,7 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     p.res = reinterpret_cast<const __half*>(d->res);
     p.ldr = d->ldr;
     p.acc_scale = d->acc_scale;
-    p.flags = d->flags;
+    p.geglu = geglu ? 1 : 0;
     p.ln_stats = reinterpret_cast<const float2*>(d->ln_stats);
     p.ln_u = d->ln_u;
     p.ln_nslots = d->ln_stats ? d->ln_nslots : 0;
@@ -1250,6 +550,8 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     p.ln_inv_c = 1.0f / (float)d->a_C;
     p.row_stats = reinterpret_cast<float2*>(d->row_stats);
     p.row_stats_slots = d->row_stats_slots;
+    p.ws_ticket = reinterpret_cast<unsigned int*>(d->workspace);
+    p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<char*>(d->workspace) + TC_GEMM_WS_TICKET_BYTES);
 
     // --- tensor maps
     {
@@ -1260,148 +562,45 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
         if (!m) return TC_ERR_CUDA;
         p.tmA = *m;
     }
-    const long long pair_tiles = (long long)((p.tiles_m + 1) / 2) * p.tiles_nn;
     {
+        // BNp rows per box: rows past the tile (or past b_rows, zero-filled) feed accumulator columns that are not stored
         uint64_t dims[2] = {(uint64_t)d->taps * (uint64_t)d->a_C, (uint64_t)d->b_rows};
         uint64_t strides[1] = {(uint64_t)d->ldb * 2};
-        uint32_t box[2] = {(uint32_t)kBlockK, (uint32_t)(pair ? BN / 2 : BN)};
+        uint32_t box[2] = {(uint32_t)kBlockK, (uint32_t)BNp};
         const CUtensorMap* m = get_tensor_map(d->b, 2, dims, strides, box);
         if (!m) return TC_ERR_CUDA;
         p.tmB = *m;
     }
 
-    const int main_kblocks = d->taps * (d->a_C / kBlockK);
-    // residual through the tensor core (extra A-only k-blocks against a shared-memory identity) unless it must stay
-    // outside the accumulator scaling
-    static const char* resmma_env = getenv("TC_GEMM_RES_MMA");   // "0" disables (A/B testing)
-    if (d->res && !geglu && d->acc_scale == 1.0f && d->n_cols % 8 == 0 && !(resmma_env && resmma_env[0] == '0')) {
-        p.res_kblocks = (BN + kBlockK - 1) / kBlockK;
-        uint64_t rdims[4] = {(uint64_t)d->n_cols, (uint64_t)d->oW, (uint64_t)d->oH, (uint64_t)d->oN};
-        uint64_t rstr[3] = {(uint64_t)d->ldr * 2, (uint64_t)d->oW * (uint64_t)d->ldr * 2,
-                            (uint64_t)d->oH * (uint64_t)d->oW * (uint64_t)d->ldr * 2};
-        uint32_t rbox[4] = {(uint32_t)kBlockK, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TN};
-        const CUtensorMap* mr = get_tensor_map(d->res, 4, rdims, rstr, rbox);
-        if (!mr) return TC_ERR_CUDA;
-        p.tmR = *mr;
-    }
-    // TMA-store epilogue: whole 32-column chunks of 16-byte-aligned rows
-    {
-        const int width = geglu ? BN / 2 : BN;
-        const int out_cols = geglu ? d->n_cols / 2 : d->n_cols;
-        static const char* tmast_env = getenv("TC_GEMM_TMA_STORE");   // "0" disables (A/B testing)
-        if (d->n_cols % 16 == 0 && width % 32 == 0 && out_cols % width == 0 && !(tmast_env && tmast_env[0] == '0')) {
-            uint64_t odims[4] = {(uint64_t)out_cols, (uint64_t)d->oW, (uint64_t)d->oH, (uint64_t)d->oN};
-            uint64_t ostr[3] = {(uint64_t)d->ldc * 2, (uint64_t)d->oW * (uint64_t)d->ldc * 2,
-                                (uint64_t)d->oH * (uint64_t)d->oW * (uint64_t)d->ldc * 2};
-            uint32_t obox[4] = {32u, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TN};
-            const CUtensorMap* mo = get_tensor_map(d->out, 4, odims, ostr, obox, 64);
-            if (!mo) return TC_ERR_CUDA;
-            p.tmO = *mo;
-            p.tma_store = 1;
-            // do the 32 rows of an epilogue warp form a box of the output tensor?
-            int wbW = 0, wbH = 0, wbN = 0;
-            if (p.TW % 32 == 0) {
-                wbW = 32, wbH = 1, wbN = 1;
-            } else if (32 % p.TW == 0) {
-                const int rows = 32 / p.TW;
-                if (p.TH % rows == 0) wbW = p.TW, wbH = rows, wbN = 1;
-                else if (rows % p.TH == 0 && p.TN % (rows / p.TH) == 0) wbW = p.TW, wbH = p.TH, wbN = rows / p.TH;
-            }
-            static const char* wbox_env = getenv("TC_GEMM_WARP_BOX");   // "0" disables (A/B testing)
-            if (wbW && (p.TW * p.TH * p.TN) % 32 == 0 && !(wbox_env && wbox_env[0] == '0')) {
-                uint32_t wbox[4] = {32u, (uint32_t)wbW, (uint32_t)wbH, (uint32_t)wbN};
-                const CUtensorMap* mw = get_tensor_map(d->out, 4, odims, ostr, wbox, 64);
-                if (!mw) return TC_ERR_CUDA;
-                p.tmOw = *mw;
-                p.warp_box = 1;
-            }
-        }
-    }
-    if (!p.tma_store) p.ksplit = 1;
-    p.kb_per = (main_kblocks + p.ksplit - 1) / p.ksplit;
-    p.fd_ks = make_fastdiv((uint32_t)p.ksplit);
-    p.fd_kc = make_fastdiv((uint32_t)p.kc_per_tap);
-    p.ws_ticket = reinterpret_cast<unsigned int*>(d->workspace);
-    p.ws_partial = reinterpret_cast<float*>(reinterpret_cast<char*>(d->workspace) + TC_GEMM_WS_TICKET_BYTES);
-    const int stage_bytes = kAStageBytes + (pair ? BN / 2 : BN) * 128;
-    // a second staging box pays off where the epilogue bounds the tile time (short K loops); long K loops would rather
-    // have the 16 KiB as operand pipeline depth (conv 320->320 lost 10 % when it went from 5 to 4 stages)
-    p.stage_bufs = (p.tma_store && d->taps * (d->a_C / kBlockK) <= 12) ? 2 : 1;
-    {
-        static const char* bs_env = getenv("TC_GEMM_BATCH_STORE");   // "0" disables (A/B testing)
-        const int width = geglu ? BN / 2 : BN;
-        const int chunks_per_group = (width / 32 + 1) / 2;
-        if (p.stage_bufs == 2 && p.ksplit == 1 && chunks_per_group <= 4 && !(bs_env && bs_env[0] == '0')) {
-            p.batch_store = 1;
-            p.stage_bufs = chunks_per_group;
-        }
-    }
-    // alignment slack, barriers, epilogue vectors, store staging, identity tile, row-statistics hand-over
-    const int kFixedSmem = 1024 + 512 + 4096 + 1024 + 16384 * p.stage_bufs + 8192 + 2048;
+    // shared memory: operand ring (at least as large as the fp32 staging tile it becomes), barriers, per-column vectors,
+    // row-statistics hand-over, alignment slack
+    const int stage_bytes = kAStageBytes + (int)p.b_bytes;
+    const int staging_bytes = kBlockM * (BNp + 4) * 4;
+    const int kFixedSmem = 1024 + 8 * 2 * 8 + 2048 + 1024 + 64;
     const int smem_budget = 227 * 1024 - kFixedSmem;
     int stages = smem_budget / stage_bytes;
     if (stages > 8) stages = 8;
-    // weight-resident mode: short K loops whose N tile fits beside >= 5 A stages, when a CTA sees several M tiles
-    static const char* bres_env = getenv("TC_GEMM_BRES");   // "0" disables (A/B testing)
-    {
-        const long long units = pair ? pair_tiles : (long long)p.tiles_m * p.tiles_nn;
-        const int slots = pair ? sm_count() / 2 : sm_count();
-        // (split-K launches never qualify: they are chosen when there are too FEW tiles per SM)
-        const int bres_bytes = main_kblocks * (pair ? BN / 2 : BN) * 128;
-        const int a_stages = (smem_budget - bres_bytes) / kAStageBytes;
-        if (bres_bytes < smem_budget && a_stages >= 5 && units >= 3LL * slots && p.ksplit == 1 && !(bres_env && bres_env[0] == '0')) {
-            p.b_resident = 1;
-            stages = a_stages > 12 ? 12 : a_stages;
-        }
-    }
     if (stages < 2) return fail(TC_ERR_INVALID, "tc_conv_gemm: not enough shared memory for 2 stages");
     p.stages = stages;
-    const size_t smem_bytes = (p.b_resident ? (size_t)stages * kAStageBytes + (size_t)main_kblocks * (pair ? BN / 2 : BN) * 128
-                                            : (size_t)stages * stage_bytes) + kFixedSmem;
+    const int ring = stages * stage_bytes > staging_bytes ? stages * stage_bytes : staging_bytes;
+    p.ring_bytes = (uint32_t)ring;
+    const size_t smem_bytes = (size_t)ring + kFixedSmem;
+    TC_CHECK_ARG(smem_bytes <= 227 * 1024, "tc_conv_gemm: tile does not fit in shared memory");
 
-    const int epi = !p.tma_store ? 2 : (geglu ? 1 : 0);
-    if (p.row_stats && epi != 0) return fail(TC_ERR_INVALID, "tc_conv_gemm: row_stats needs the TMA-store epilogue (n_cols % 16 == 0, block_n % 32 == 0)");
-    using KernelFn = void (*)(GemmKParams);
-    static const KernelFn kernels[2][3] = {
-        {tc_gemm_kernel<false, 0>, tc_gemm_kernel<false, 1>, tc_gemm_kernel<false, 2>},
-        {tc_gemm_kernel<true, 0>, tc_gemm_kernel<true, 1>, tc_gemm_kernel<true, 2>}};
     static bool attr_set = false;
     if (!attr_set) {
-        for (int a = 0; a < 2; ++a)
-            for (int b = 0; b < 3; ++b) {
-                int rc = check_cuda(cudaFuncSetAttribute(reinterpret_cast<const void*>(kernels[a][b]),
-                                                         cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
-                                    "cudaFuncSetAttribute(tc_gemm_kernel)");
-                if (rc) return rc;
-            }
+        for (int i = 0; i < 8; ++i) {
+            int rc = check_cuda(cudaFuncSetAttribute(reinterpret_cast<const void*>(kKernels[i]),
+                                                     cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024),
+                                "cudaFuncSetAttribute(tc_gemm_kernel)");
+            if (rc) return rc;
+        }
         attr_set = true;
     }
-    int units = pair ? sm_count() / 2 : sm_count();
-    {
-        const long long total_units = (pair ? pair_tiles : (long long)p.tiles_m * p.tiles_nn) * p.ksplit;
-        if (total_units < units) units = (int)total_units;
-        // N-tile-fastest raster (see TC_DECODE_TILE).  With resident weights the unit count must be a multiple of tiles_nn
-        // (then unit u keeps N tile u % tiles_nn for its whole life); give up at most ~4 % of the SMs for that.
-        static const char* raster_env = getenv("TC_GEMM_RASTER");   // "0" keeps the N-major order (A/B testing)
-        if (p.tiles_nn > 1 && total_units > units && !(raster_env && raster_env[0] == '0')) {
-            const int rounded = units - units % p.tiles_nn;
-            if (rounded > 0 && (units - rounded) * 25 <= units) {
-                units = rounded;
-                p.raster = 1;
-            } else if (!p.b_resident) {
-                p.raster = 1;
-            }
-        }
-    }
-    p.fd_nn = make_fastdiv((uint32_t)p.tiles_nn);
-    p.fd_mu = make_fastdiv((uint32_t)(pair ? (p.tiles_m + 1) / 2 : p.tiles_m));
-    p.fd_x = make_fastdiv((uint32_t)p.tiles_x);
-    p.fd_y = make_fastdiv((uint32_t)p.tiles_y);
-    p.fd_xy = make_fastdiv((uint32_t)(p.tiles_x * p.tiles_y));
-    p.fd_b2 = make_fastdiv((uint32_t)p.bias2_rows_per);
-    const int grid = pair ? 2 * units : units;
-    g_last_cfg[0] = BN, g_last_cfg[1] = pair ? 1 : 0, g_last_cfg[2] = p.ksplit, g_last_cfg[3] = stages;
-    launch(kernels[pair ? 1 : 0][epi], dim3(grid), dim3(kThreads), smem_bytes, stream, pair ? 2 : 1, p);
+    const long long grid = tiles_m * p.tiles_nn * p.ksplit;
+    TC_CHECK_ARG(grid < (1LL << 31), "tc_conv_gemm: too many tiles");
+    g_last_cfg[0] = BN, g_last_cfg[1] = 0, g_last_cfg[2] = p.ksplit, g_last_cfg[3] = stages;
+    launch(kKernels[BNp / 32 - 1], dim3((unsigned)grid), dim3(kThreads), smem_bytes, stream, 1, p);
     count_launch();
     TC_CHECK_LAUNCH("tc_gemm_kernel launch");
     return TC_OK;

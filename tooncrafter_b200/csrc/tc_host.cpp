@@ -33,7 +33,7 @@ int sm_count() {
             cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
             cached = n;
         else
-            cached = 148;
+            cached = 132;
     }
     return cached;
 }

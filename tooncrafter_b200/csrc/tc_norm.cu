@@ -81,8 +81,8 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, long long ldx, lon
         mine[C + v * 8 + i] = sq[i];
     }
     __syncthreads();
-    // block reduction in a fixed order (deterministic), one warp per (group, sum | sumsq) task: 32 threads walking
-    // rows_per_iter x cpg values serially cost ~3.7 us per launch, most of a small tensor's GroupNorm
+    // block reduction in a fixed order (deterministic), one warp per (group, sum | sumsq) task rather than 32 threads
+    // walking rows_per_iter x cpg values serially
     const int cpg = C / G;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     const int n = rows_per_iter * cpg;
@@ -177,8 +177,8 @@ __global__ void gn_apply_kernel(const __half* __restrict__ x, long long ldx, __h
 }
 
 // ---- single-pass GroupNorm for small / medium tensors: one CTA (or a cluster of 2-8 CTAs) per (stat group, norm group) -----
-// The two-kernel path costs ~5 us of launch / tail per kernel plus two reads of the tensor: 12-23 us (back to back) for the
-// 3-13 MB activations of UNet levels 2 and 3 (77 of the 166 GroupNorms of a forward); this kernel 8-18 us.  Here the unit's elements — `cpg` contiguous
+// The two-kernel path pays two launches and two reads of the tensor, which dominate for the few-MB activations of UNet
+// levels 2 and 3 (77 of the 166 GroupNorms of a forward).  Here the unit's elements — `cpg` contiguous
 // channels of every pixel of the stat group — are loaded ONCE into registers (kVec-byte vectors, at most kMaxV per thread),
 // reduced (warp shuffles -> shared memory -> fixed-order sum; across a cluster through distributed shared memory, summed in
 // rank order: deterministic), normalised (+SiLU) in registers and stored.  One read, one write, one launch.
@@ -457,7 +457,7 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
             if (threads >= 32 && total_v <= 8LL * threads * kMaxV) {
                 int csize = 1;
                 while ((long long)csize * threads * kMaxV < total_v + (long long)csize * (vpp + 1)) ++csize;   // whole pixels per CTA
-                // (26 MB tensors in 512 one-per-SM CTAs = 3.5 waves measured 43 us against 26 us on the two-kernel path)
+                // (a large tensor would need several waves of one-per-SM CTAs: it stays on the two-kernel path)
                 const long long n_units = (long long)n_stat * G;
                 if (csize <= 8 && (csize == 1 || n_units * csize <= 2LL * sm_count())) {
                     // small units: shrink the block to what the unit needs (several units resident per SM); with many units
@@ -488,7 +488,7 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
     // one round of 4 loads per thread allows; large ones are capped to one resident wave below
     long long want = (pps + (long long)k * 4 - 1) / ((long long)k * 4);
     int nblk = (int)(want < 1 ? 1 : want);
-    // exactly one resident wave (2 blocks of <= 512 threads per SM): 320 blocks on 296 slots ran as two waves
+    // exactly one resident wave (2 blocks of <= 512 threads per SM): one block more than that runs as two waves
     int cap = (2 * sm_count()) / n_stat;
     if (cap < 1) cap = 1;
     if (cap > kGnMaxPartials) cap = kGnMaxPartials;

@@ -1,5 +1,5 @@
 """Inference-side mirror of the reference's model objects (the Python surface scripts/evaluation/inference.py,
-scripts/evaluation/funcs.py and gradio_app.py touch — SURVEY §8b "B1"), backed by the CUDA engines.
+scripts/evaluation/funcs.py and gradio_app.py touch), backed by the CUDA engines.
 
 Mirrors (interface, attribute names, buffer names, semantics; paths relative to /root/reference):
   DDPM / LatentDiffusion / LatentVisualDiffusion   lvdm/models/ddpm3d.py:41-187, 465-560, 598-683, 735-750, 1041-1062
@@ -7,7 +7,7 @@ Mirrors (interface, attribute names, buffer names, semantics; paths relative to 
   AutoencoderKL / AutoencoderKL_Dualref            lvdm/models/autoencoder.py:13-116, 238-258
   DiagonalGaussianDistribution                     lvdm/distributions.py:24-64
   instantiate_from_config                          utils/utils.py:27-42
-Training/logging methods of the reference classes are out of scope (SURVEY §2 #15).
+Training/logging methods of the reference classes are out of scope.
 """
 from __future__ import annotations
 
@@ -137,8 +137,7 @@ class AutoencoderKL(nn.Module):
         """kwargs: ref_context (5 maps [b, C, 2, H, W]) and timesteps, as decode_core passes them."""
         from .vae_engine import DecoderEngine
         if len(kwargs) == 0:
-            raise NotImplementedError("decode() without ref_context/timesteps never happens on the VideoDecoder path "
-                                      "(SURVEY App. C.2)")
+            raise NotImplementedError("decode() without ref_context/timesteps never happens on the VideoDecoder path")
         from . import runtime
         ex = runtime.TEST_EXECUTOR
         if self._dec_engine is None or not self._dec_engine.matches(self.decoder):
@@ -146,7 +145,7 @@ class AutoencoderKL(nn.Module):
         ref = kwargs.get("ref_context")
         T = kwargs.get("timesteps") or z.shape[0]
         if z.shape[0] != T:
-            raise NotImplementedError("one clip per decode call (the reference mixes clips for B > 1, SURVEY App. C.3)")
+            raise NotImplementedError("one clip per decode call (the reference mixes clips for B > 1)")
         return self._dec_engine.decode(z.float(), ref, executor=ex).clone()
 
 
@@ -297,7 +296,7 @@ class LatentVisualDiffusion(nn.Module):
             z = z.permute(0, 2, 1, 3, 4).reshape(b * t, z.shape[1], *z.shape[3:])
         z = 1.0 / self.scale_factor * z
         if not self.perframe_ae:
-            raise NotImplementedError("VideoDecoder needs the chunked (perframe_ae=True) path (SURVEY App. C.2)")
+            raise NotImplementedError("VideoDecoder needs the chunked (perframe_ae=True) path")
         n = self.en_and_decode_n_samples_a_time or self.temporal_length
         outs = []
         for i in range(0, z.shape[0], n):

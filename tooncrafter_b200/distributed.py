@@ -1,10 +1,10 @@
-"""Multi-GPU plumbing.  Throughput mode — the clip-parallel path (SURVEY §8e): the reference shards prompts across ranks with no
+"""Multi-GPU plumbing.  Throughput mode — the clip-parallel path: the reference shards prompts across ranks with no
 collective on the data path (scripts/evaluation/inference.py:314-320, scripts/evaluation/ddp_wrapper.py:8-46).
 
 One process per GPU; the only collectives are ONE broadcast of the weights at init and the max-over-ranks of the
 timed region.  Backend "nccl" on GPUs (NVLink 5 / NVSwitch), "gloo" in the CPU tests.
 
-Latency mode (SURVEY §8f-4, optional): pairs of adjacent ranks share ONE clip.  Classifier-free guidance needs two UNet
+Latency mode: pairs of adjacent ranks share ONE clip.  Classifier-free guidance needs two UNet
 evaluations per step (ddim.py:217-232); pair-rank 0 runs the conditional branch, pair-rank 1 the unconditional one
 (B = 1 each instead of one B = 2 forward), and one NCCL all-gather of the two fp16 predictions (2 x 327 KB at 320x512x16)
 per DDIM step is the only exchange: both ranks then apply the identical fused DDIM update.  `latency_pairs()` builds the

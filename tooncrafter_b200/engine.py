@@ -6,7 +6,7 @@ Reference semantics restated by the builders (paths relative to /root/reference)
   ResBlock / TemporalConvBlock           openaimodel3d.py:210-236, 272-279
   SpatialTransformer / TemporalTransformer / BasicTransformerBlock / CrossAttention / GEGLU-FF
                                          lvdm/modules/attention.py:81-144, 242-246, 294-310, 365-412, 415-442
-B200-first departures (results identical up to fp16 rounding):
+H100-first departures (results identical up to fp16 rounding):
   * channels-last [B][T][H][W][C] fp16 activations; no layout copies, skip "cat" realised by writing producers
     straight into channel slices of the concat buffer;
   * cond / uncond batched as B = 2 through one forward; context K/V projections computed once per
@@ -448,7 +448,7 @@ class UNetEngine:
         if n_ctx != 77 + 16 * T:
             raise NotImplementedError("context must hold 77 text + 16 image tokens per frame "
                                       "(openaimodel3d.py:556 hard-codes this layout)")
-        # arena: generous static budget (activations of one B-sample forward), see DESIGN.md
+        # arena: generous static budget (activations of one B-sample forward)
         px = N * H * W
         arena_bytes = self.arena_bytes or int(px * lay.model_channels * 2 * 40 + (256 << 20))
         arena = Arena(arena_bytes, dev)

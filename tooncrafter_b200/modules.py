@@ -263,7 +263,7 @@ class Encoder(nn.Module):
 class Resampler(nn.Module):
     """Drop-in for lvdm.modules.encoders.resampler.Resampler (same ctor kwargs, same state-dict keys): the perceiver
     resampler that turns CLIP image tokens into the 16 x T image-context tokens of the UNet's cross-attention
-    (SURVEY 8f-2; reference resampler.py:96-145, PerceiverAttention :49-93, FeedForward :27-34)."""
+    (reference resampler.py:96-145, PerceiverAttention :49-93, FeedForward :27-34)."""
 
     def __init__(self, dim=1024, depth=8, dim_head=64, heads=16, num_queries=8, embedding_dim=768, output_dim=1024,
                  ff_mult=4, video_length=None):

@@ -1,7 +1,7 @@
 """Torch-tensor wrappers over the C ABI (include/tooncrafter_b200.h).
 
 torch is plumbing only here: it owns device memory and the current stream; every op below is one (or a few)
-launches of our own sm_100a kernels through ctypes.  There is no fallback path — a missing library raises.
+launches of our own sm_90a kernels through ctypes.  There is no fallback path — a missing library raises.
 """
 from __future__ import annotations
 

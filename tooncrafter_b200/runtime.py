@@ -1,6 +1,6 @@
 """Host runtime shared by the UNet and VAE engines: activation pool, activation views, recorded programs.
 
-Design (B200-first): every network is executed as a STATIC program — a flat list of C-ABI kernel launches over
+Design (H100-first): every network is executed as a STATIC program — a flat list of C-ABI kernel launches over
 pre-allocated channels-last fp16 buffers carved out of one HBM arena — built once per input geometry and then
 replayed, either launch-by-launch or as a captured CUDA graph (no per-step Python/allocator work, no
 `rearrange().contiguous()` copies: spatial tokens, temporal tokens and conv pixels are all views of the same

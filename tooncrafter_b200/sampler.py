@@ -1,4 +1,4 @@
-"""DDIMSampler with the reference's public API (lvdm/models/samplers/ddim.py:10-279), B200-native inside.
+"""DDIMSampler with the reference's public API (lvdm/models/samplers/ddim.py:10-279), H100-native inside.
 
 Fast path (the configuration scripts/run.sh uses: v-parameterisation, classifier-free guidance with a conditioning
 dict, no mask / corrector / quantiser): per step ONE batched UNet program replay (cond and uncond rows as B = 2b,
@@ -50,7 +50,7 @@ class DDIMSampler(object):
     def __init__(self, model, schedule="linear", **kwargs):
         super().__init__()
         # optional: a 2-rank torch.distributed group (distributed.latency_pairs()); the fused path then evaluates one
-        # guidance branch per rank and all-gathers the two predictions every step (SURVEY 8f-4)
+        # guidance branch per rank and all-gathers the two predictions every step
         self.latency_group = None
         # tests only: interpret the engine's recorded programs and the fused update on the PyTorch emulator (no GPU)
         from . import runtime
@@ -365,7 +365,7 @@ class DDIMSamplerMultiCond(DDIMSampler):
 
     Fused path (same option set as DDIMSampler's): the three branches run as ONE B = 3b UNet program per step and
     tc_ddim_step3 does the three-way combine, guidance rescale and update.  Other option combinations take the
-    general path below: three passes through the CUDA UNet engine + torch elementwise plumbing (SURVEY 8f-3)."""
+    general path below: three passes through the CUDA UNet engine + torch elementwise plumbing."""
 
     def _fast_path_ok(self, cond, uc, cfg_scale, mask, quantize, corrector, noise_dropout, precision, orig_steps,
                       shape, kwargs=None):

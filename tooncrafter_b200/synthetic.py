@@ -6,7 +6,7 @@ iteration order or on which other tensors exist, and the GPU box regenerates bit
 A freshly constructed reference model is useless for parity: every block's last layer is zero-initialised
 (openaimodel3d.py:179,269-270,381-382,545; attention.py:288-290,360-362; autoencoder_dualref.py:261-262,348-349,
 640), so the UNet output is identically 0 and every transformer/temporal block is the identity.  Here all of
-them get non-zero values (SURVEY §8d).
+them get non-zero values.
 """
 from __future__ import annotations
 

@@ -8,10 +8,10 @@ Reference semantics restated (paths relative to /root/reference):
   Combiner (levels 0, 1 and before conv_out)                      :357-368
   AE3DConv (conv_out + time_mix_conv)                             :929-935
   AutoencoderKL.decode skips post_quant_conv when kwargs are given  lvdm/models/autoencoder.py:112-116
-One call decodes ONE chunk of T latents of ONE clip (the only case in which the reference is well defined,
-SURVEY App. C.2/C.3); the T = 16 and T = 14 passes of scripts/evaluation/inference.py:262-270 use two plans.
+One call decodes ONE chunk of T latents of ONE clip (the only case in which the reference is well defined);
+the T = 16 and T = 14 passes of scripts/evaluation/inference.py:262-270 use two plans.
 
-B200-first notes: the learned alpha-blend of VideoResBlock is folded into the last temporal conv's epilogue
+H100-first notes: the learned alpha-blend of VideoResBlock is folded into the last temporal conv's epilogue
 (out = s + sigmoid(mix) * h), the Combiner's add is the residual of its own 1x1-conv GEMM written in place,
 reference-frame K/V projections are computed once per clip, and the mid-block softmax bias trick
 (P (V + 1 b^T) = P V + b^T) lets V^T be produced directly by a GEMM.
@@ -312,7 +312,7 @@ def taps_3x3_stride2_pad_br(n_frames: int):
 
 
 class EncoderEngine:
-    """AutoencoderKL.encode(x, return_hidden_states=True): Encoder + quant_conv (SURVEY §8f-1, "next" row).
+    """AutoencoderKL.encode(x, return_hidden_states=True): Encoder + quant_conv.
 
     Reference: lvdm/modules/networks/ae_modules.py:432-475 (Encoder.forward), :153-213 (ResnetBlock), :28-75
     (AttnBlock), :92-108 (Downsample, asymmetric pad); lvdm/models/autoencoder.py:100-105 (quant_conv)."""
