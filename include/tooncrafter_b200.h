@@ -138,11 +138,13 @@ int tc_layernorm(const void* x, long long ldx, void* y, long long ldy, const flo
                  int rows, int C, float eps, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
- * Fused attention, head dim 64, on mma.sync tensor-core MMAs (QK^T and PV), online softmax in fp32.
- * q:  [q_batches][Lq][heads*64] (row stride ldq), kv segment s: k/v [kv_batches_s][Lk_s][heads*64].
+ * Fused attention, head dim 64 (or 80), on mma.sync tensor-core MMAs (QK^T and PV), online softmax in fp32.
+ * q:  [q_batches][Lq][heads*D] (row stride ldq), kv segment s: k/v [kv_batches_s][Lk_s][heads*D], D = head dim.
  * Query batch b attends to kv batch b / kv_div[s].  With two segments the two softmax-attention
  * results are summed (text + image cross attention, attention.py:128-142,153-207); with one it is plain
  * attention (attention.py:103-120,175; autoencoder_dualref.py:270-341).
+ * head_dim 80 (the OpenCLIP ViT-H/14 vision tower: 16 heads of 80) and causal = 1 (key j masked for query i when
+ * j > i: the OpenCLIP text tower's attn_mask) take one segment.  Both fields 0 = head dim 64, no mask.
  */
 typedef struct {
   const void* q; long long ldq; int q_batches; int Lq; int heads;
@@ -150,6 +152,8 @@ typedef struct {
   const void* k[2]; const void* v[2]; long long ldk[2]; long long ldv[2]; int Lk[2]; int kv_div[2];
   void* out; long long ldo;
   float scale;
+  int head_dim; /* 0 or 64, or 80 */
+  int causal;   /* 0 or 1 */
 } TcAttention;
 int tc_attention(const TcAttention* desc, void* stream);
 

@@ -59,6 +59,7 @@ class TcAttention(C.Structure):
         ("Lk", C.c_int * 2), ("kv_div", C.c_int * 2),
         ("out", C.c_void_p), ("ldo", C.c_longlong),
         ("scale", C.c_float),
+        ("head_dim", C.c_int), ("causal", C.c_int),
     ]
 
 

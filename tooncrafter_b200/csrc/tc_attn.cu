@@ -1,7 +1,9 @@
 // tooncrafter_b200 — attention kernels.
 //
 //  tc_attention           fused softmax(QK^T)V, head dim 64, one or two key/value segments (each with its own softmax,
-//                         outputs summed), mma.sync m16n8k16 with fp32 accumulators and an fp32 online softmax.
+//                         outputs summed), mma.sync m16n8k16 with fp32 accumulators and an fp32 online softmax; one
+//                         segment may also take head dim 80 (OpenCLIP ViT-H/14 vision tower) and a causal mask (its
+//                         text tower).
 //  tc_attention_wide      the same kernel for one head of up to 512 channels (VAE mid-block attention): scores stay
 //                         on chip; each CTA produces 256, 128 or 64 of the value channels (the widest that divides D).
 //  tc_temporal_attention  16-frame temporal self-attention, one (pixel, head) per warp, mma.sync 16x8x16 (HBM-bound).
@@ -51,6 +53,7 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 // Flash-style: a CTA of 4 warps takes 64 query rows (16 per warp) of one (batch, head, value chunk); key tiles of 64
 // rows are staged in shared memory (K and V loads in separate cp.async groups, so S = Q K^T runs while V arrives).
 // Rows of D halfs are stored with their 16-byte chunks XOR-swizzled by (row & 7) so ldmatrix rows hit distinct banks.
+// The XOR needs 8k chunks per row; 80-wide rows (10 chunks) use a padded row stride of 11 chunks instead (tile_off).
 constexpr int kFaRows = 64;
 constexpr int kFaKeys = 64;
 constexpr int kFaThreads = 128;
@@ -78,16 +81,31 @@ struct FaParams {
 // byte offset of 16-byte chunk c of row r in a swizzled tile with `cpr` chunks per row
 __device__ __forceinline__ uint32_t swz(int r, int c, int cpr) { return (uint32_t)((r * cpr + (c ^ (r & 7))) << 4); }
 
-// kTwoSeg: up to two key/value segments, each with its own softmax, outputs summed (a second accumulator set)
-template <int kDV, bool kTwoSeg>
+// Tile layout of the head-dim-80 instance (10 chunks per row): rows padded to 11 chunks (176 bytes), no XOR.  An
+// ldmatrix phase reads one 16-byte chunk from each of 8 consecutive rows r..r+7 at the same column; their chunk indices
+// 11 r + c fall in bank groups (11 r + c) mod 8, and since 11 is odd, r -> 11 r mod 8 is a bijection on 8 consecutive
+// rows: the 8 reads hit 8 distinct 16-byte bank groups (conflict-free).
+constexpr int kPadCpr = 11;
+template <int kDV>
+__device__ __forceinline__ uint32_t tile_off(int r, int c, int cpr) {
+    if constexpr (kDV == 80) return (uint32_t)((r * kPadCpr + c) << 4);
+    else return swz(r, c, cpr);
+}
+// shared-memory bytes of one tile of `rows` rows of D halfs
+__host__ __device__ constexpr int tile_bytes(int rows, int D) { return D == 80 ? rows * kPadCpr * 16 : rows * D * 2; }
+
+// kTwoSeg: up to two key/value segments, each with its own softmax, outputs summed (a second accumulator set).
+// kDV = 80: head dim 80 for q / k and v (single segment).  kCausal: key j is masked for query i when j > i, and key
+// tiles wholly above the diagonal of this CTA's query rows are skipped.
+template <int kDV, bool kTwoSeg, bool kCausal>
 __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p) {
     tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
     extern __shared__ __align__(128) uint8_t fa_smem[];
     const int D = p.D, cq = D / 8;                 // 16-byte chunks per q / k row
     constexpr int cv = kDV / 8;                    // 16-byte chunks per v row
     const uint32_t sQ = tc::smem_u32(fa_smem);
-    const uint32_t sK = sQ + (uint32_t)(kFaRows * D * 2);
-    const uint32_t sV = sK + (uint32_t)(kFaKeys * D * 2);
+    const uint32_t sK = sQ + (uint32_t)(kDV == 80 ? tile_bytes(kFaRows, 80) : kFaRows * D * 2);
+    const uint32_t sV = sK + (uint32_t)(kDV == 80 ? tile_bytes(kFaKeys, 80) : kFaKeys * D * 2);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int q0 = blockIdx.x * kFaRows;
     const int head = blockIdx.y / p.nv, vchunk = blockIdx.y - head * p.nv;
@@ -99,7 +117,7 @@ __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p
         const int r = i / cq, c = i - r * cq;
         const bool ok = q0 + r < p.Lq;
         const __half* src = p.q + ((long long)b * p.Lq + (ok ? q0 + r : 0)) * p.ldq + qk_col + c * 8;
-        cp_async16(sQ + swz(r, c, cq), src, ok);
+        cp_async16(sQ + tile_off<kDV>(r, c, cq), src, ok);
     }
     cp_async_commit();
 
@@ -115,18 +133,20 @@ __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p
 #pragma unroll
         for (int j = 0; j < kDV / 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
         float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
-        for (int k0 = 0; k0 < sg.Lk; k0 += kFaKeys) {
+        // causal: keys beyond this CTA's last query row are masked for every row of the CTA
+        const int k_end = kCausal ? min(sg.Lk, q0 + kFaRows) : sg.Lk;
+        for (int k0 = 0; k0 < k_end; k0 += kFaKeys) {
             __syncthreads();   // every warp is done with the previous K / V tile
             for (int i = tid; i < kFaKeys * cq; i += kFaThreads) {
                 const int r = i / cq, c = i - r * cq;
                 const bool ok = k0 + r < sg.Lk;
-                cp_async16(sK + swz(r, c, cq), sg.k + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldk + qk_col + c * 8, ok);
+                cp_async16(sK + tile_off<kDV>(r, c, cq), sg.k + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldk + qk_col + c * 8, ok);
             }
             cp_async_commit();
             for (int i = tid; i < kFaKeys * cv; i += kFaThreads) {
                 const int r = i / cv, c = i - r * cv;
                 const bool ok = k0 + r < sg.Lk;
-                cp_async16(sV + swz(r, c, cv), sg.v + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldv + v_col + c * 8, ok);
+                cp_async16(sV + tile_off<kDV>(r, c, cv), sg.v + (kvb * sg.Lk + (ok ? k0 + r : 0)) * sg.ldv + v_col + c * 8, ok);
             }
             cp_async_commit();
             cp_async_wait<1>();   // Q and K have landed
@@ -138,24 +158,28 @@ __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p
             for (int j = 0; j < 8; ++j) sc[j][0] = sc[j][1] = sc[j][2] = sc[j][3] = 0.f;
             for (int kk = 0; kk < D / 16; ++kk) {
                 uint32_t a[4];
-                ldsm_x4(sQ + swz(warp * 16 + (lane & 15), 2 * kk + (lane >> 4), cq), a[0], a[1], a[2], a[3]);
+                ldsm_x4(sQ + tile_off<kDV>(warp * 16 + (lane & 15), 2 * kk + (lane >> 4), cq), a[0], a[1], a[2], a[3]);
 #pragma unroll
                 for (int np = 0; np < 4; ++np) {
                     uint32_t b0, b1, b2, b3;
-                    ldsm_x4(sK + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), 2 * kk + ((lane >> 3) & 1), cq), b0, b1, b2, b3);
+                    ldsm_x4(sK + tile_off<kDV>(np * 16 + (lane & 7) + ((lane >> 4) << 3), 2 * kk + ((lane >> 3) & 1), cq), b0, b1, b2, b3);
                     mma_m16n8k16(sc[2 * np], a, b0, b1);
                     mma_m16n8k16(sc[2 * np + 1], a, b2, b3);
                 }
             }
             // ---- online softmax (rows g and g + 8 of the warp; a row lives in the 4 lanes of a quad)
             float mx0 = m0, mx1 = m1;
+            const int qr0 = q0 + warp * 16 + g;    // query rows of sc[.][0..1] and sc[.][2..3]: qr0, qr0 + 8
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
 #pragma unroll
                 for (int i = 0; i < 2; ++i) {
-                    const bool key_ok = k0 + 8 * j + 2 * t4 + i < sg.Lk;
-                    sc[j][i] = key_ok ? sc[j][i] * p.scale_log2 : -INFINITY;
-                    sc[j][2 + i] = key_ok ? sc[j][2 + i] * p.scale_log2 : -INFINITY;
+                    const int key = k0 + 8 * j + 2 * t4 + i;
+                    const bool key_ok = key < sg.Lk;
+                    const bool ok0 = key_ok && (!kCausal || key <= qr0);
+                    const bool ok1 = key_ok && (!kCausal || key <= qr0 + 8);
+                    sc[j][i] = ok0 ? sc[j][i] * p.scale_log2 : -INFINITY;
+                    sc[j][2 + i] = ok1 ? sc[j][2 + i] * p.scale_log2 : -INFINITY;
                     mx0 = fmaxf(mx0, sc[j][i]);
                     mx1 = fmaxf(mx1, sc[j][2 + i]);
                 }
@@ -199,7 +223,7 @@ __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p
 #pragma unroll
                 for (int nd = 0; nd < kDV / 8; nd += 2) {
                     uint32_t b0, b1, b2, b3;
-                    ldsm_x4_t(sV + swz(mrow, nd + (lane >> 4), cv), b0, b1, b2, b3);
+                    ldsm_x4_t(sV + tile_off<kDV>(mrow, nd + (lane >> 4), cv), b0, b1, b2, b3);
                     if (p.split_p) {
                         mma_m16n8k16(o[nd], pl, b0, b1);
                         mma_m16n8k16(o[nd + 1], pl, b2, b3);
@@ -516,28 +540,34 @@ __global__ void softmax_rows_kernel(__half* __restrict__ s, long long lds, int r
 
 using namespace tc_host;
 
-template <int kDV, bool kTwoSeg>
+template <int kDV, bool kTwoSeg, bool kCausal = false>
 static int launch_flash_kernel(const FaParams& p, dim3 grid, size_t smem_bytes, cudaStream_t stream) {
     static bool attr_set = false;
     if (!attr_set) {
-        int rc = check_cuda(cudaFuncSetAttribute(flash_attn_kernel<kDV, kTwoSeg>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        int rc = check_cuda(cudaFuncSetAttribute(flash_attn_kernel<kDV, kTwoSeg, kCausal>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                  227 * 1024),
                             "cudaFuncSetAttribute(flash_attn_kernel)");
         if (rc) return rc;
         attr_set = true;
     }
-    tc_host::launch(flash_attn_kernel<kDV, kTwoSeg>, grid, dim3(kFaThreads), smem_bytes, stream, 1, p);
+    tc_host::launch(flash_attn_kernel<kDV, kTwoSeg, kCausal>, grid, dim3(kFaThreads), smem_bytes, stream, 1, p);
     return TC_OK;
 }
 
 // split_p: P as fp16 hi + lo parts for the PV product when few keys average its rounding (cross attention: 77 + 16 keys)
-static int launch_flash(const FaParams& p0, int batches, int Lk_max, cudaStream_t stream) {
+static int launch_flash(const FaParams& p0, int batches, int Lk_max, bool causal, cudaStream_t stream) {
     FaParams p = p0;
     p.split_p = Lk_max <= 512 ? 1 : 0;
-    const size_t smem_bytes = (size_t)(2 * kFaRows * p.D + kFaKeys * p.DV) * 2 + 128;
+    // Q and K tiles of D halfs per row, V tile of DV halfs per row (80-wide rows padded to 11 chunks, tile_off)
+    const size_t smem_bytes = (size_t)(tile_bytes(kFaRows, p.D) + tile_bytes(kFaKeys, p.D) + tile_bytes(kFaKeys, p.DV)) + 128;
     dim3 grid((p.Lq + kFaRows - 1) / kFaRows, p.heads * p.nv, batches);
     int rc;
-    if (p.n_seg == 2)
+    if (p.D == 80)                                                              // tc_attention only: DV = D = 80
+        rc = causal ? launch_flash_kernel<80, false, true>(p, grid, smem_bytes, stream)
+                    : launch_flash_kernel<80, false, false>(p, grid, smem_bytes, stream);
+    else if (causal)                                                            // tc_attention only: DV = D = 64
+        rc = launch_flash_kernel<64, false, true>(p, grid, smem_bytes, stream);
+    else if (p.n_seg == 2)
         rc = launch_flash_kernel<64, true>(p, grid, smem_bytes, stream);        // tc_attention only: DV = D = 64
     else if (p.DV == 64)
         rc = launch_flash_kernel<64, false>(p, grid, smem_bytes, stream);
@@ -559,6 +589,11 @@ extern "C" int tc_attention(const TcAttention* d, void* stream_v) {
     TC_CHECK_ARG(d->ldq % 8 == 0 && d->ldo % 8 == 0, "tc_attention: strides must be multiples of 8");
     TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(d->q) | reinterpret_cast<uintptr_t>(d->out)) & 15) == 0,
                  "tc_attention: operands must be 16-byte aligned");
+    TC_CHECK_ARG(d->head_dim == 0 || d->head_dim == 64 || d->head_dim == 80, "tc_attention: head_dim must be 0, 64 or 80");
+    TC_CHECK_ARG(d->causal == 0 || d->causal == 1, "tc_attention: causal must be 0 or 1");
+    const int D = d->head_dim == 80 ? 80 : 64;
+    TC_CHECK_ARG(d->n_seg == 1 || (D == 64 && !d->causal),
+                 "tc_attention: head dim 80 and causal masking take one key/value segment");
     FaParams p;
     memset(&p, 0, sizeof(p));
     int Lk_max = 0;
@@ -579,14 +614,14 @@ extern "C" int tc_attention(const TcAttention* d, void* stream_v) {
     p.ldq = d->ldq;
     p.Lq = d->Lq;
     p.heads = d->heads;
-    p.D = 64;
-    p.DV = 64;
+    p.D = D;
+    p.DV = D;
     p.nv = 1;
     p.n_seg = d->n_seg;
     p.out = reinterpret_cast<__half*>(d->out);
     p.ldo = d->ldo;
     p.scale_log2 = d->scale * 1.4426950408889634f;
-    return launch_flash(p, d->q_batches, Lk_max, stream);
+    return launch_flash(p, d->q_batches, Lk_max, d->causal != 0, stream);
 }
 
 extern "C" int tc_attention_wide(const void* q, const void* k, const void* v, long long ldq, long long ldk, long long ldv,
@@ -621,7 +656,7 @@ extern "C" int tc_attention_wide(const void* q, const void* k, const void* v, lo
     p.out = reinterpret_cast<__half*>(out);
     p.ldo = ldo;
     p.scale_log2 = scale * 1.4426950408889634f;
-    return launch_flash(p, batches, Lk, stream);
+    return launch_flash(p, batches, Lk, false, stream);
 }
 
 extern "C" int tc_debug_read_attn_trace(unsigned long long* host_dst, int count) {

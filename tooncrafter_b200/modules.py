@@ -293,3 +293,228 @@ class Resampler(nn.Module):
         if self._engine is None or not self._engine.matches(self):
             self._engine = ResamplerEngine(self)
         return self._engine.forward(x).clone()
+
+
+# ------------------------------------------------------------------------- conditioning: OpenCLIP text / image towers
+# Geometry of the OpenCLIP architectures the reference configs name (configs/inference_512_v1.0.yaml: "ViT-H-14").
+# `arch` may also be a dict of the same form (width-reduced test models).
+CLIP_ARCHS = {
+    "ViT-H-14": dict(embed_dim=1024,
+                     text=dict(width=1024, heads=16, layers=24, ctx=77, vocab=49408),
+                     vision=dict(width=1280, heads=16, layers=32, patch=14, image=224)),
+}
+CLIP_SOT, CLIP_EOT = 49406, 49407                    # open_clip's <start_of_text> / <end_of_text> token ids
+CLIP_MEAN = (0.48145466, 0.4578275, 0.40821073)      # reference condition.py:318-319
+CLIP_STD = (0.26862954, 0.26130258, 0.27577711)
+
+
+def _clip_arch(arch):
+    if isinstance(arch, dict):
+        return arch
+    if arch not in CLIP_ARCHS:
+        raise NotImplementedError(f"OpenCLIP arch {arch!r} is not supported (supported: {sorted(CLIP_ARCHS)})")
+    return CLIP_ARCHS[arch]
+
+
+def _param(*shape):
+    return nn.Parameter(torch.empty(shape), requires_grad=False)
+
+
+def _clip_linear(cin, cout, bias=True):
+    n = Node()
+    n.register_parameter("weight", _param(cout, cin))
+    if bias:
+        n.register_parameter("bias", _param(cout))
+    return n
+
+
+def _clip_ln(c):
+    n = Node()
+    n.register_parameter("weight", _param(c))
+    n.register_parameter("bias", _param(c))
+    return n
+
+
+def _clip_transformer(width, layers):
+    """open_clip.transformer.Transformer: pre-LayerNorm residual attention blocks (nn.MultiheadAttention with a fused
+    in_proj, MLP c_fc -> GELU (erf) -> c_proj, 4x wide)."""
+    blocks = nn.ModuleList()
+    for _ in range(layers):
+        attn = Node(out_proj=_clip_linear(width, width))
+        attn.register_parameter("in_proj_weight", _param(3 * width, width))
+        attn.register_parameter("in_proj_bias", _param(3 * width))
+        blocks.append(Node(ln_1=_clip_ln(width), attn=attn, ln_2=_clip_ln(width),
+                           mlp=Node(c_fc=_clip_linear(width, 4 * width), c_proj=_clip_linear(4 * width, width))))
+    return Node(resblocks=blocks)
+
+
+def _clip_text_top(model: Node, a) -> None:
+    """Text-side top-level tensors of open_clip's CLIP module (the transformer itself is added by the text class)."""
+    t = a["text"]
+    model.put("token_embedding", Node())
+    model.token_embedding.register_parameter("weight", _param(t["vocab"], t["width"]))
+    model.register_parameter("positional_embedding", _param(t["ctx"], t["width"]))
+    model.put("ln_final", _clip_ln(t["width"]))
+    model.register_parameter("text_projection", _param(t["width"], a["embed_dim"]))
+    model.register_parameter("logit_scale", _param())
+    # causal mask of the text tower (open_clip CLIP.build_attention_mask); non-persistent, as in open_clip
+    model.register_buffer("attn_mask", torch.full((t["ctx"], t["ctx"]), float("-inf")).triu_(1), persistent=False)
+
+
+def clip_tokenize(text, ctx: int = 77) -> torch.Tensor:
+    """Token ids [B, ctx] of a list of strings.  Uses open_clip.tokenize when open_clip imports; without it only the
+    empty prompt is known (<start_of_text> <end_of_text> then zeros: what image_guided_synthesis feeds the
+    unconditional branch and every prompt when text input is off)."""
+    if isinstance(text, str):
+        text = [text]
+    try:
+        import open_clip
+    except ImportError:
+        open_clip = None
+    if open_clip is not None:
+        return open_clip.tokenize(list(text), context_length=ctx)
+    out = torch.zeros(len(text), ctx, dtype=torch.long)
+    for i, s in enumerate(text):
+        if s != "":
+            raise RuntimeError(f"tokenizing {s!r} needs open_clip's BPE tokenizer (open_clip.tokenize), which is not "
+                               "installed; without it only the empty prompt \"\" is supported, or pass token ids [B, 77]")
+        out[i, 0], out[i, 1] = CLIP_SOT, CLIP_EOT
+    return out
+
+
+def _gaussian_blur_reflect(x: torch.Tensor, sigma, ksize) -> torch.Tensor:
+    """Separable Gaussian blur with reflect borders (kornia.filters.gaussian_blur2d)."""
+    for axis, (s, k) in enumerate(zip(sigma, ksize)):
+        r = torch.arange(k, dtype=torch.float32, device=x.device) - (k - 1) / 2
+        w = torch.exp(-r * r / (2.0 * s * s))
+        w = (w / w.sum()).to(x.dtype)
+        C = x.shape[1]
+        if axis == 0:      # along H
+            x = torch.nn.functional.pad(x, (0, 0, k // 2, k // 2), mode="reflect")
+            x = torch.nn.functional.conv2d(x, w.view(1, 1, k, 1).repeat(C, 1, 1, 1), groups=C)
+        else:              # along W
+            x = torch.nn.functional.pad(x, (k // 2, k // 2, 0, 0), mode="reflect")
+            x = torch.nn.functional.conv2d(x, w.view(1, 1, 1, k).repeat(C, 1, 1, 1), groups=C)
+    return x
+
+
+def clip_preprocess(x: torch.Tensor, size: int = 224, antialias: bool = True) -> torch.Tensor:
+    """Reference condition.py:322-330: kornia.geometry.resize(x, (size, size), interpolation="bicubic",
+    align_corners=True, antialias) -> (x + 1) / 2 -> CLIP mean / std normalisation; x in [-1, 1], [B, 3, H, W].
+
+    The resize is restated from kornia's published algorithm (kornia is not a dependency here, so it is not checked
+    against kornia itself): when an axis is downscaled by `factor` and antialias is on, a Gaussian blur with
+    sigma = max((factor - 1) / 2, 0.001) per axis, a kernel of int(max(4 sigma, 3)) taps (made odd) and reflect
+    borders on both axes, then bicubic interpolation with align_corners=True."""
+    x = x.float()
+    H, W = x.shape[-2:]
+    if antialias and max(H / size, W / size) > 1:
+        sig = (max((H / size - 1.0) / 2.0, 0.001), max((W / size - 1.0) / 2.0, 0.001))
+        ks = tuple(k + 1 if k % 2 == 0 else k for k in (int(max(4.0 * s, 3)) for s in sig))
+        x = _gaussian_blur_reflect(x, sig, ks)
+    x = torch.nn.functional.interpolate(x, size=(size, size), mode="bicubic", align_corners=True)
+    x = (x + 1.0) / 2.0
+    mean = torch.tensor(CLIP_MEAN, device=x.device).view(1, 3, 1, 1)
+    std = torch.tensor(CLIP_STD, device=x.device).view(1, 3, 1, 1)
+    return (x - mean) / std
+
+
+def _clip_engine(module, cls):
+    from . import runtime
+    ex = runtime.TEST_EXECUTOR
+    if module._engine is None or not module._engine.matches(module):
+        module._engine = cls(module, plan_only=ex is not None)
+    return ex
+
+
+class FrozenOpenCLIPEmbedder(nn.Module):
+    """Drop-in for lvdm.modules.encoders.condition.FrozenOpenCLIPEmbedder (same ctor kwargs; state-dict keys those of
+    open_clip's CLIP after `del model.visual`, reference condition.py:184-202).  Downloads nothing: the parameters
+    are empty until the checkpoint's cond_stage_model.* tensors are loaded.  forward / encode run the text tower on
+    the CUDA engine (reference :209-231) and return [B, 77, width] fp32 after ln_final."""
+
+    LAYERS = ["last", "penultimate"]
+
+    def __init__(self, arch="ViT-H-14", version="laion2b_s32b_b79k", device="cuda", max_length=77, freeze=True,
+                 layer="last"):
+        super().__init__()
+        if layer not in self.LAYERS:
+            raise NotImplementedError(f"layer must be one of {self.LAYERS}, got {layer!r}")
+        a = _clip_arch(arch)
+        t = a["text"]
+        self.arch, self.version, self.device, self.max_length = arch, version, device, max_length
+        self.heads = t["heads"]
+        self.layer = layer
+        self.layer_idx = 0 if layer == "last" else 1
+        self.model = Node()
+        _clip_text_top(self.model, a)
+        self.model.put("transformer", _clip_transformer(t["width"], t["layers"]))
+        self._engine = None
+        if freeze:
+            self.freeze()
+
+    def freeze(self):
+        self.eval()
+        for p in self.parameters():
+            p.requires_grad = False
+
+    def tokenize(self, text) -> torch.Tensor:
+        return clip_tokenize(text, self.model.positional_embedding.shape[0])
+
+    def forward(self, text):
+        """text: list of strings (or one string), or token ids [B, 77] -> [B, 77, width] fp32."""
+        tokens = text if isinstance(text, torch.Tensor) else self.tokenize(text)
+        from .cond_engine import ClipTextEngine
+        ex = _clip_engine(self, ClipTextEngine)
+        return self._engine.forward(tokens, executor=ex).clone()
+
+    def encode(self, text):
+        return self(text)
+
+
+class FrozenOpenCLIPImageEmbedderV2(nn.Module):
+    """Drop-in for lvdm.modules.encoders.condition.FrozenOpenCLIPImageEmbedderV2 (same ctor kwargs; state-dict keys
+    those of open_clip's CLIP after `del model.transformer`, reference condition.py:300-320).  Downloads nothing.
+    forward: images [B, 3, H, W] in [-1, 1] -> the vision transformer's [B, 1 + grid^2, width] tokens, fp32, without
+    ln_post or proj (reference :337-372), on the CUDA engine."""
+
+    def __init__(self, arch="ViT-H-14", version="laion2b_s32b_b79k", device="cuda", freeze=True, layer="pooled",
+                 antialias=True):
+        super().__init__()
+        if layer != "pooled":
+            raise NotImplementedError(f"layer must be 'pooled', got {layer!r}")    # reference condition.py:312-314
+        a = _clip_arch(arch)
+        v = a["vision"]
+        self.arch, self.version, self.device, self.layer, self.antialias = arch, version, device, layer, antialias
+        self.heads, self.patch, self.image_size = v["heads"], v["patch"], v["image"]
+        grid, w = v["image"] // v["patch"], v["width"]
+        self.model = Node()
+        _clip_text_top(self.model, a)
+        visual = Node(conv1=Node(), ln_pre=_clip_ln(w), transformer=_clip_transformer(w, v["layers"]),
+                      ln_post=_clip_ln(w))
+        visual.register_parameter("class_embedding", _param(w))
+        visual.register_parameter("positional_embedding", _param(grid * grid + 1, w))
+        visual.register_parameter("proj", _param(w, a["embed_dim"]))
+        visual.conv1.register_parameter("weight", _param(w, 3, v["patch"], v["patch"]))
+        self.model.put("visual", visual)
+        self.register_buffer("mean", torch.tensor(CLIP_MEAN), persistent=False)
+        self.register_buffer("std", torch.tensor(CLIP_STD), persistent=False)
+        self._engine = None
+        if freeze:
+            self.freeze()
+
+    def freeze(self):
+        self.eval()
+        for p in self.model.parameters():
+            p.requires_grad = False
+
+    def preprocess(self, x):
+        return clip_preprocess(x, self.image_size, self.antialias)
+
+    def forward(self, image, no_dropout=False):
+        from .cond_engine import ClipImageEngine
+        ex = _clip_engine(self, ClipImageEngine)
+        return self._engine.forward(self.preprocess(image), executor=ex).clone()
+
+    def encode(self, image):
+        return self(image)

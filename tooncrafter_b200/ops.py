@@ -186,8 +186,11 @@ def layernorm(x: torch.Tensor, y: torch.Tensor, gamma: torch.Tensor, beta: torch
 
 
 def attention(q: torch.Tensor, segs, out: torch.Tensor, *, q_batches: int, Lq: int, heads: int, scale: float,
-              ldq: int, ldo: int, q_offset: int = 0, out_offset: int = 0) -> None:
-    """segs: list of dicts {k, v, ldk, ldv, Lk, kv_div, k_offset, v_offset} (1 or 2 segments)."""
+              ldq: int, ldo: int, q_offset: int = 0, out_offset: int = 0, head_dim: int = 64,
+              causal: bool = False) -> None:
+    """segs: list of dicts {k, v, ldk, ldv, Lk, kv_div, k_offset, v_offset} (1 or 2 segments).
+
+    head_dim 64 or 80; causal masks key j for query i when j > i.  Head dim 80 and causal take one segment."""
     _req_half(q, "q"); _req_half(out, "out")
     lib = _lib.load()
     d = TcAttention()
@@ -203,6 +206,8 @@ def attention(q: torch.Tensor, segs, out: torch.Tensor, *, q_batches: int, Lq: i
     d.out = out.data_ptr() + 2 * out_offset
     d.ldo = ldo
     d.scale = scale
+    d.head_dim = head_dim
+    d.causal = 1 if causal else 0
     check(lib.tc_attention(C.byref(d), _stream()), "tc_attention")
 
 
