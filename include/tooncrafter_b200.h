@@ -197,6 +197,14 @@ int tc_add2d(const void* x, long long ldx, void* y, long long ldy, long long row
  * y may alias x */
 int tc_gelu2d(const void* x, long long ldx, void* y, long long ldy, long long rows, int cols, void* stream);
 
+/* One interpolated segment into the joined uint8 video (scripts/evaluation/inference.py:148-153, 262-270):
+ * x16: the decoder's fp16 [T][3][H][W] output of the 16-frame pass; x14: NULL or the [T-2][3][H][W] output of the
+ * 14-frame pass of the same clip, whose frames T/2-2 and T/2-1 replace frames T/2-1 and T/2 (the middle-frame splice).
+ * Frames f_begin <= f < f_end are written to out[f - f_begin][H][W][3] (uint8, NTHWC; `out` points at the first of
+ * them) as u = (uint8)(((clamp(x, -1, 1) + 1) / 2) * 255), fp32 ops in that order, truncation toward zero.
+ * Any H, W; the vectorised path needs H*W % 8 == 0, 16-byte aligned inputs and an 8-byte aligned `out`. */
+int tc_video_u8(const void* x16, const void* x14, int T, int H, int W, int f_begin, int f_end, void* out, void* stream);
+
 /* sinusoidal embedding (utils_diffusion.py:8-28) + Linear -> SiLU -> Linear MLP (openaimodel3d.py:370-382,550-577):
  * out[b][:] (+)= W2 * silu(W1 * sincos(t[b]) + b1) + b2, fp32 output.  dim = model_channels. */
 int tc_time_embed(const float* t, int B, int dim, const void* w1, const float* b1, const void* w2, const float* b2,

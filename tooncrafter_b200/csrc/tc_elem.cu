@@ -359,6 +359,62 @@ __global__ void ddim_update_kernel(const __half* __restrict__ e_c, const __half*
     }
 }
 
+// ------------------------------------------------------------------------------------------------ video output
+// One channel value of the reference's save path (inference.py:148-153), in torch's fp32 op order with no contraction:
+// clamp(x, -1, 1) -> (v + 1) / 2 -> v * 255 -> uint8 (truncation toward zero; v is in [0, 255]).
+__device__ __forceinline__ uint32_t to_u8(__half h) {
+    float v = fminf(fmaxf(__half2float(h), -1.0f), 1.0f);
+    v = __fdiv_rn(__fadd_rn(v, 1.0f), 2.0f);
+    v = __fmul_rn(v, 255.0f);
+    return __float2uint_rz(v);
+}
+
+// Output frame f (of [f_begin, f_end)) of one segment, written as out[f - f_begin][p][c] (NTHWC uint8).  Source: the
+// 16-frame decode x16 [T][3][HW], except frames T/2-1 and T/2, which come from frames T/2-2 and T/2-1 of the 14-frame
+// decode x14 [T-2][3][HW] when it is given (inference.py:270).  One thread per group of 8 pixels of one frame: with
+// vec, three 16-byte channel-plane loads and three 8-byte stores of the 24 packed bytes; otherwise a scalar loop.
+__global__ void video_u8_kernel(const __half* __restrict__ x16, const __half* __restrict__ x14, int T, long long HW,
+                                int f_begin, int n_frames, uint8_t* __restrict__ out, int vec) {
+    tc::pdl_wait();
+    const long long groups = (HW + 7) / 8;
+    const long long total = groups * n_frames;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int fo = (int)(i / groups);
+        const long long p0 = (i - (long long)fo * groups) * 8;
+        const int f = f_begin + fo;
+        const bool mid = x14 != nullptr && (f == T / 2 - 1 || f == T / 2);
+        const __half* src = mid ? x14 + (long long)(f - 1) * 3 * HW : x16 + (long long)f * 3 * HW;
+        uint8_t* dst = out + ((long long)fo * HW + p0) * 3;
+        if (vec) {
+            uint4 c[3];
+#pragma unroll
+            for (int ch = 0; ch < 3; ++ch) c[ch] = ld16(src + ch * HW + p0);
+            const __half* h0 = reinterpret_cast<const __half*>(&c[0]);
+            const __half* h1 = reinterpret_cast<const __half*>(&c[1]);
+            const __half* h2 = reinterpret_cast<const __half*>(&c[2]);
+            uint32_t w[6] = {0, 0, 0, 0, 0, 0};
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const uint32_t u[3] = {to_u8(h0[k]), to_u8(h1[k]), to_u8(h2[k])};
+#pragma unroll
+                for (int ch = 0; ch < 3; ++ch) {
+                    const int b = 3 * k + ch;                  // byte b of the 24 packed bytes
+                    w[b >> 2] |= u[ch] << (8 * (b & 3));
+                }
+            }
+            uint2* d2 = reinterpret_cast<uint2*>(dst);
+            d2[0] = make_uint2(w[0], w[1]);
+            d2[1] = make_uint2(w[2], w[3]);
+            d2[2] = make_uint2(w[4], w[5]);
+        } else {
+            const int np = (int)min(8LL, HW - p0);
+            for (int k = 0; k < np; ++k)
+                for (int ch = 0; ch < 3; ++ch) dst[3 * k + ch] = (uint8_t)to_u8(src[ch * HW + p0 + k]);
+        }
+    }
+}
+
 inline int grid_for(long long total, int threads, int max_blocks) {
     long long g = (total + threads - 1) / threads;
     if (g > max_blocks) g = max_blocks;
@@ -500,6 +556,24 @@ extern "C" int tc_small_linear(const float* x, int B, int K, const void* w, cons
                                                             reinterpret_cast<__half*>(y), ldy, silu_in, 0);
     count_launch();
     TC_CHECK_LAUNCH("small_linear_kernel");
+    return TC_OK;
+}
+
+extern "C" int tc_video_u8(const void* x16, const void* x14, int T, int H, int W, int f_begin, int f_end, void* out,
+                           void* stream_v) {
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    TC_CHECK_ARG(x16 && out && T > 0 && H > 0 && W > 0, "tc_video_u8: bad arguments");
+    TC_CHECK_ARG(0 <= f_begin && f_begin < f_end && f_end <= T, "tc_video_u8: frame window must satisfy 0 <= f_begin < f_end <= T");
+    TC_CHECK_ARG(!x14 || (T >= 4 && T % 2 == 0), "tc_video_u8: the middle-frame splice needs an even T >= 4");
+    const long long HW = (long long)H * W;
+    const int vec = HW % 8 == 0 && (reinterpret_cast<uintptr_t>(x16) & 15) == 0 &&
+                    (reinterpret_cast<uintptr_t>(x14) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0;
+    const long long total = (HW + 7) / 8 * (f_end - f_begin);
+    tc_host::launch(video_u8_kernel, dim3(grid_for(total, 256, 16 * sm_count())), dim3(256), 0, stream, 1,
+                    reinterpret_cast<const __half*>(x16), reinterpret_cast<const __half*>(x14), T, HW, f_begin,
+                    f_end - f_begin, reinterpret_cast<uint8_t*>(out), vec);
+    count_launch();
+    TC_CHECK_LAUNCH("video_u8_kernel");
     return TC_OK;
 }
 

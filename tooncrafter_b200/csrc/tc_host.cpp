@@ -146,7 +146,7 @@ bool pdl_enabled() {
 
 extern "C" {
 const char* tc_last_error(void) { return tc_host::g_err.c_str(); }
-int tc_version(void) { return 101; }
+int tc_version(void) { return 102; }
 unsigned long long tc_launch_count(void) { return tc_host::g_launches.load(); }
 int tc_sm_count(void) { return tc_host::sm_count(); }
 }

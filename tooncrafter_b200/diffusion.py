@@ -148,6 +148,15 @@ class AutoencoderKL(nn.Module):
             raise NotImplementedError("one clip per decode call (the reference mixes clips for B > 1)")
         return self._dec_engine.decode(z.float(), ref, executor=ex).clone()
 
+    def decoder_engine(self):
+        """The DecoderEngine decode() runs on (built on first use).  Its decode() returns a view of the plan's static
+        output buffer, valid until the next decode of the same T: for callers that consume it in place."""
+        from . import runtime
+        from .vae_engine import DecoderEngine
+        if self._dec_engine is None or not self._dec_engine.matches(self.decoder):
+            self._dec_engine = DecoderEngine(self.decoder, plan_only=runtime.TEST_EXECUTOR is not None)
+        return self._dec_engine
+
 
 class AutoencoderKL_Dualref(AutoencoderKL):
     def _make_decoder(self, dd):

@@ -290,9 +290,8 @@ class Resampler(nn.Module):
     def forward(self, x):
         """x [B, n_tokens, embedding_dim] (CLIP image tokens) -> [B, num_queries (* video_length), output_dim] fp32."""
         from .cond_engine import ResamplerEngine
-        if self._engine is None or not self._engine.matches(self):
-            self._engine = ResamplerEngine(self)
-        return self._engine.forward(x).clone()
+        ex = _clip_engine(self, ResamplerEngine)
+        return self._engine.forward(x, executor=ex).clone()
 
 
 # ------------------------------------------------------------------------- conditioning: OpenCLIP text / image towers

@@ -279,6 +279,29 @@ def gelu2d(x, y, *, rows, cols, ldx, ldy, x_offset=0, y_offset=0) -> None:
           "tc_gelu2d")
 
 
+def video_u8(x16: torch.Tensor, x14: Optional[torch.Tensor], out: torch.Tensor, *, f_begin: int, f_end: int,
+             out_frame: int) -> None:
+    """Frames [f_begin, f_end) of one segment -> out[out_frame + f - f_begin] (uint8 [F, H, W, 3]).
+
+    x16: fp16 [T, 3, H, W] decoder output of the 16-frame pass; x14: None or the [T-2, 3, H, W] output of the
+    14-frame pass, whose frames T/2-2, T/2-1 replace frames T/2-1, T/2.  u = uint8(((clamp(x, -1, 1) + 1) / 2) * 255)."""
+    _req_half(x16, "x16")
+    T, C3, H, W = x16.shape
+    if C3 != 3 or not x16.is_contiguous():
+        raise ValueError("video_u8: x16 must be a contiguous [T, 3, H, W] tensor")
+    if x14 is not None:
+        _req_half(x14, "x14")
+        if tuple(x14.shape) != (T - 2, 3, H, W) or not x14.is_contiguous():
+            raise ValueError(f"video_u8: x14 must be a contiguous [{T - 2}, 3, {H}, {W}] tensor")
+    if out.dtype != torch.uint8 or not out.is_cuda or not out.is_contiguous() or tuple(out.shape[1:]) != (H, W, 3):
+        raise ValueError(f"video_u8: out must be a contiguous CUDA uint8 [F, {H}, {W}, 3] tensor")
+    if out_frame < 0 or out_frame + (f_end - f_begin) > out.shape[0]:
+        raise ValueError("video_u8: the frame window does not fit the output")
+    lib = _lib.load()
+    check(lib.tc_video_u8(x16.data_ptr(), _ptr(x14), T, H, W, f_begin, f_end, out.data_ptr() + out_frame * H * W * 3,
+                          _stream()), "tc_video_u8")
+
+
 def time_embed(t: torch.Tensor, w1, b1, w2, b2, out: torch.Tensor, ws: torch.Tensor, *, dim: int, hidden: int,
                accumulate: bool) -> None:
     lib = _lib.load()

@@ -1,0 +1,183 @@
+"""Keyframe interpolation end to end: K >= 2 keyframes -> one joined uint8 video.
+
+The reference turns ONE pair of keyframes into a 16-frame clip with its evaluation glue (scripts/evaluation/inference.py:
+load_data_prompts :64-106, image_guided_synthesis :180-277, save_results_seperate :135-155).  `ToonCrafterPipeline`
+restates that glue on this library for a storyboard of K keyframes: S = K - 1 segments (S = K with `loop`, the last
+one running from keyframe K-1 back to keyframe 0), sampled together and joined into one video.
+
+Per call:
+  * preprocessing of load_data_prompts (shorter side resized to min(size) with anti-aliasing, centre crop, [-1, 1]) as
+    torchvision tensor ops on the model's device;
+  * ONE VAE encode of the K distinct keyframes (the reference encodes 8 copies of each frame of a pair); segment k
+    gets c_concat = z_k at frame 0, z_{k+1} at frame T-1, zeros elsewhere (inference.py:197-200), and the decoder
+    reference maps [h_k, h_{k+1}] per level (inference.py:164-178);
+  * ONE image-tower pass over the first keyframe of every segment plus the zero image, ONE text-tower pass over the
+    distinct prompts plus "" (inference.py:186-216);
+  * the segments as the batch rows of one fused DDIM sample() per group of `segments_per_batch`;
+  * per segment the T = 16 and T = 14 decodes (inference.py:262-270), read in place by one tc_video_u8 launch that
+    applies the middle-frame splice and the uint8 conversion of the save path and writes the segment's frames into
+    the joined video at frame (T-1)*k.
+
+RNG contract: keyframe j's posterior noise is drawn from a CPU generator seeded `seed + j`; segment k's x_T and
+DDIM step noise come from a generator on the model's device seeded `seed + k` (DDIMSampler's `noise_generators`).
+So segment k of a K-keyframe run is the same computation as a 2-keyframe run on (keyframe k, keyframe k+1) with
+`seed + k`, whatever batch it runs in (up to the batch tiling of the kernels).
+
+Seam rule: neighbouring segments share a keyframe; the earlier segment's last frame is kept and the later segment's
+frame 0 is dropped.  With `loop`, the closing segment's last frame (keyframe 0 again) is dropped as well, so the
+video has (T-1)*S + 1 frames, or (T-1)*K with `loop`.
+"""
+from __future__ import annotations
+
+from typing import Sequence, Union
+
+import numpy as np
+import torch
+
+from . import ops, runtime
+from .modules import clip_tokenize
+from .sampler import DDIMSampler, DDIMSamplerMultiCond
+
+
+def preprocess(keyframes, size=(320, 512), device="cpu") -> torch.Tensor:
+    """uint8 HWC RGB images -> [K, 3, size[0], size[1]] float32 in [-1, 1] on `device`.
+
+    load_data_prompts's transform (inference.py:65-69): Resize(min(size)) (shorter side, bilinear, anti-aliased),
+    CenterCrop(size) (zero padding where the image is smaller), ToTensor, Normalize(0.5, 0.5).  The resize runs on the
+    uint8 tensor, like PIL's; an image whose shorter side already is min(size) is not resampled."""
+    from torchvision.transforms.v2 import functional as TF
+    if isinstance(keyframes, (torch.Tensor, np.ndarray)) and keyframes.ndim == 4:
+        keyframes = list(keyframes)
+    out = []
+    for im in keyframes:
+        t = im if isinstance(im, torch.Tensor) else torch.from_numpy(np.array(im))
+        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[-1] != 3:
+            raise ValueError(f"keyframes must be uint8 [H, W, 3] RGB images, got {t.dtype} {tuple(t.shape)}")
+        t = t.to(device).permute(2, 0, 1)
+        if min(t.shape[1:]) != min(size):
+            t = TF.resize(t, min(size), antialias=True)
+        if tuple(t.shape[1:]) != tuple(size):
+            t = TF.center_crop(t, list(size))
+        out.append(t)
+    return torch.stack(out).float().div(255).sub(0.5).div(0.5)
+
+
+class ToonCrafterPipeline:
+    """K keyframes -> one interpolated video, on a LatentVisualDiffusion of this library (see the module docstring)."""
+
+    def __init__(self, model):
+        self.model = model
+
+    def _text(self, prompts, S: int):
+        """(per-segment text embeddings [S, 77, D], the embedding of "" [1, 77, D]) from one text-tower pass."""
+        m = self.model
+        if isinstance(prompts, torch.Tensor):
+            if prompts.dim() != 2 or prompts.shape[0] != S:
+                raise ValueError(f"token ids must be [S={S}, 77], got {tuple(prompts.shape)}")
+            uniq, inv = torch.unique(prompts.long().cpu(), dim=0, return_inverse=True)
+            emb = m.get_learned_conditioning(torch.cat([uniq, clip_tokenize([""], prompts.shape[1])]).to(m.device))
+            return emb[inv.to(emb.device)], emb[-1:]
+        texts = [prompts] * S if isinstance(prompts, str) else list(prompts)
+        if len(texts) != S:
+            raise ValueError(f"{len(texts)} prompts for {S} segments")
+        distinct = list(dict.fromkeys(texts + [""]))
+        emb = m.get_learned_conditioning(distinct)
+        idx = torch.tensor([distinct.index(t) for t in texts], device=emb.device)
+        return emb[idx], emb[distinct.index("")][None]
+
+    @torch.no_grad()
+    def interpolate(self, keyframes, prompts: Union[str, Sequence[str], torch.Tensor] = "", steps: int = 50,
+                    cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
+                    timestep_spacing: str = "uniform_trailing", cfg_img=None, loop: bool = False, seed: int = 123,
+                    size=(320, 512), segments_per_batch: int = 4, output: str = "uint8") -> torch.Tensor:
+        """keyframes: K >= 2 uint8 RGB images (tensor [K, H, W, 3], ndarray, or a list of [H, W, 3] arrays of any
+        size).  prompts: one string for every segment, a list of S strings, or token ids [S, 77] (strings other than
+        "" need open_clip's tokenizer).  cfg_img not None: three-way guidance (DDIMSamplerMultiCond).  Defaults are
+        those of the reference's scripts/run.sh.
+
+        Returns uint8 [F, size[0], size[1], 3] on the model's device, F = (T-1)*S + 1 (or (T-1)*K with `loop`); with
+        output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]]."""
+        m = self.model
+        dev = m.device
+        if output not in ("uint8", "float"):
+            raise ValueError(f"output must be 'uint8' or 'float', got {output!r}")
+        if size[0] % 16 or size[1] % 16:
+            raise ValueError(f"size {tuple(size)} must be a multiple of 16")
+        if m.model.conditioning_key != "hybrid":
+            raise NotImplementedError("keyframe interpolation needs the hybrid (concat + cross-attention) model")
+        T = m.temporal_length
+        if (m.en_and_decode_n_samples_a_time or T) < T:
+            raise NotImplementedError("the pipeline decodes each segment's T frames in one call")
+        ex = runtime.TEST_EXECUTOR
+        frames = preprocess(keyframes, size, dev)
+        K = frames.shape[0]
+        if K < 2:
+            raise ValueError("interpolation needs at least two keyframes")
+        S = K if loop else K - 1
+        first = list(range(S))
+        last = [(k + 1) % K for k in range(S)]
+
+        # conditioning: text over the distinct prompts + "", image over each segment's first keyframe + the zero image
+        cond_emb, empty_emb = self._text(prompts, S)
+        if m.uncond_type == "empty_seq":
+            uc_emb = empty_emb.expand_as(cond_emb)
+        elif m.uncond_type == "zero_embed":
+            uc_emb = torch.zeros_like(cond_emb)
+        else:
+            raise NotImplementedError(f"uncond_type {m.uncond_type!r}")
+        img = torch.cat([frames[first], torch.zeros_like(frames[:1])])
+        img_all = m.image_proj_model(m.embedder(img))
+        img_emb, uc_img_emb = img_all[:S], img_all[S:].expand(S, -1, -1)
+
+        # first stage: the K distinct keyframes once; keyframe j's posterior noise from a CPU generator seeded seed + j
+        post, hidden = m.first_stage_model.encode(frames, return_hidden_states=True)
+        noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(seed + j))
+                             for j in range(K)])
+        z = m.get_first_stage_encoding(post, noise=noise)                           # [K, 4, h, w]
+        h, w = z.shape[-2:]
+        c_concat = torch.zeros(S, z.shape[1], T, h, w, dtype=z.dtype, device=dev)
+        c_concat[:, :, 0] = z[first]
+        c_concat[:, :, -1] = z[last]
+
+        F = (T - 1) * S + (0 if loop else 1)
+        video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=dev) if output == "uint8" else
+                 torch.empty(S, 3, T, size[0], size[1], dtype=torch.float32, device=dev))
+        sampler = DDIMSampler(m) if cfg_img is None else DDIMSamplerMultiCond(m)
+        dec = m.first_stage_model.decoder_engine()
+        keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
+        for g0 in range(0, S, segments_per_batch):
+            seg = list(range(g0, min(g0 + segments_per_batch, S)))
+            b = len(seg)
+            cc = [c_concat[seg]]
+            cond = {"c_crossattn": [torch.cat([cond_emb[seg], img_emb[seg]], 1)], "c_concat": cc}
+            uc = ({"c_crossattn": [torch.cat([uc_emb[seg], uc_img_emb[seg]], 1)], "c_concat": cc}
+                  if cfg_scale != 1.0 else None)
+            extra = {}
+            if cfg_img is not None:
+                extra = dict(cfg_img=cfg_img, unconditional_conditioning_img_nonetext={
+                    "c_crossattn": [torch.cat([uc_emb[seg], img_emb[seg]], 1)], "c_concat": cc})
+            gens = [torch.Generator(device=dev).manual_seed(seed + k) for k in seg]
+            samples, _ = sampler.sample(S=steps, conditioning=cond, batch_size=b, shape=[z.shape[1], T, h, w],
+                                        verbose=False, unconditional_guidance_scale=cfg_scale,
+                                        unconditional_conditioning=uc, eta=eta,
+                                        fs=torch.tensor([fs] * b, dtype=torch.long, device=dev),
+                                        timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale,
+                                        noise_generators=gens, **extra)
+            for i, k in enumerate(seg):
+                ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
+                lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
+                y16 = dec.decode(lat.float(), ref, executor=ex)                         # views of the plans' outputs
+                y14 = dec.decode(lat[keep].float(), ref, executor=ex)
+                if output == "float":
+                    v = y16.float()
+                    v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
+                    video[k] = v.permute(1, 0, 2, 3)
+                    continue
+                f_begin = 0 if k == 0 else 1
+                f_end = T - 1 if (loop and k == S - 1) else T
+                args, kw = (y16, y14, video), dict(f_begin=f_begin, f_end=f_end, out_frame=(T - 1) * k + f_begin)
+                if ex is not None:
+                    ex(ops.video_u8, args, kw)
+                else:
+                    ops.video_u8(*args, **kw)
+        return video

@@ -40,6 +40,16 @@ def make_ddim_sampling_parameters(alphacums, ddim_timesteps, eta, verbose=False)
     return sigmas, alphas, alphas_prev
 
 
+def randn_rows(shape, device, generators=None):
+    """torch.randn(shape) or, with one torch.Generator per batch row, each row drawn from its own generator (so a row's
+    noise does not depend on which batch it runs in)."""
+    if generators is None:
+        return torch.randn(shape, device=device)
+    if len(generators) != shape[0]:
+        raise ValueError(f"noise_generators: {len(generators)} generators for {shape[0]} batch rows")
+    return torch.stack([torch.randn(tuple(shape[1:]), generator=g, device=device) for g in generators])
+
+
 def rescale_noise_cfg(noise_cfg, noise_pred_text, guidance_rescale=0.0):
     dims = list(range(1, noise_pred_text.ndim))
     factor = noise_pred_text.std(dim=dims, keepdim=True) / noise_cfg.std(dim=dims, keepdim=True)
@@ -101,6 +111,10 @@ class DDIMSampler(object):
                noise_dropout=0.0, score_corrector=None, corrector_kwargs=None, verbose=True, schedule_verbose=False,
                x_T=None, log_every_t=100, unconditional_guidance_scale=1.0, unconditional_conditioning=None,
                precision=None, fs=None, timestep_spacing="uniform", guidance_rescale=0.0, **kwargs):
+        """Reference signature, plus `noise_generators`: None (the global RNG, as the reference) or one torch.Generator
+        per batch row on the model's device, from which that row's x_T (when not given) and every step's DDIM noise
+        are drawn."""
+        noise_generators = kwargs.pop("noise_generators", None)
         if conditioning is not None:
             first = conditioning[list(conditioning.keys())[0]] if isinstance(conditioning, dict) else conditioning
             cbs = (first[0] if isinstance(first, (list, tuple)) else first).shape[0]
@@ -114,7 +128,8 @@ class DDIMSampler(object):
                                   score_corrector=score_corrector, corrector_kwargs=corrector_kwargs, x_T=x_T,
                                   log_every_t=log_every_t, unconditional_guidance_scale=unconditional_guidance_scale,
                                   unconditional_conditioning=unconditional_conditioning, verbose=verbose,
-                                  precision=precision, fs=fs, guidance_rescale=guidance_rescale, **kwargs)
+                                  precision=precision, fs=fs, guidance_rescale=guidance_rescale,
+                                  noise_generators=noise_generators, **kwargs)
 
     def _fast_path_ok(self, cond, uc, cfg_scale, mask, quantize, corrector, noise_dropout, precision, orig_steps,
                       shape, kwargs=None):
@@ -131,10 +146,10 @@ class DDIMSampler(object):
                       quantize_denoised=False, mask=None, x0=None, img_callback=None, log_every_t=100,
                       temperature=1.0, noise_dropout=0.0, score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1.0, unconditional_conditioning=None, verbose=True,
-                      precision=None, fs=None, guidance_rescale=0.0, **kwargs):
+                      precision=None, fs=None, guidance_rescale=0.0, noise_generators=None, **kwargs):
         device = self.model.betas.device
         b = shape[0]
-        img = torch.randn(shape, device=device) if x_T is None else x_T
+        img = randn_rows(shape, device, noise_generators) if x_T is None else x_T
         if precision == 16:
             img = img.to(dtype=torch.float16)
         if timesteps is None:
@@ -153,7 +168,8 @@ class DDIMSampler(object):
             return self._sample_fused(self._guidance_branches(cond, unconditional_conditioning, kwargs), img,
                                       list(time_range), total_steps, unconditional_guidance_scale, guidance_rescale,
                                       temperature, fs, callback, img_callback, log_every_t, intermediates,
-                                      cfg_img=self._cfg_img(unconditional_guidance_scale, kwargs))
+                                      cfg_img=self._cfg_img(unconditional_guidance_scale, kwargs),
+                                      noise_generators=noise_generators)
 
         for i, step in enumerate(time_range):
             index = total_steps - i - 1
@@ -168,7 +184,8 @@ class DDIMSampler(object):
                                               corrector_kwargs=corrector_kwargs,
                                               unconditional_guidance_scale=unconditional_guidance_scale,
                                               unconditional_conditioning=unconditional_conditioning, mask=mask, x0=x0,
-                                              fs=fs, guidance_rescale=guidance_rescale, **kwargs)
+                                              fs=fs, guidance_rescale=guidance_rescale,
+                                              noise_generators=noise_generators, **kwargs)
             if callback:
                 callback(i)
             if img_callback:
@@ -280,7 +297,7 @@ class DDIMSampler(object):
             st.ex(fn, args, dict(B=b, n=st.n))
 
     def _sample_fused(self, branches, img, time_range, total_steps, cfg_scale, phi, temperature, fs, callback,
-                      img_callback, log_every_t, intermediates, cfg_img=None):
+                      img_callback, log_every_t, intermediates, cfg_img=None, noise_generators=None):
         steps = [(total_steps - i - 1, time_range[i]) for i in range(total_steps)]
         st = self._fused_setup(branches[0], branches[1], tuple(img.shape), steps, cfg_scale, phi, temperature, fs,
                                extra_branches=tuple(branches[2:]), cfg_img=cfg_img)
@@ -291,7 +308,7 @@ class DDIMSampler(object):
             from .distributed import sync_pair_state
             sync_pair_state(x, st.group)                                   # same x_T and same noise stream on both ranks
         for i, (index, _) in enumerate(steps):
-            noise = torch.randn(x.shape, device=st.dev)                    # one draw per step, as ddim.py:273
+            noise = randn_rows(x.shape, st.dev, noise_generators)          # one draw per step, as ddim.py:273
             self._fused_step(st, i, x, noise, x_next, pred_x0)
             x, x_next = x_next, x
             if callback:
@@ -308,7 +325,8 @@ class DDIMSampler(object):
     def p_sample_ddim(self, x, c, t, index, repeat_noise=False, use_original_steps=False, quantize_denoised=False,
                       temperature=1.0, noise_dropout=0.0, score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1.0, unconditional_conditioning=None, uc_type=None,
-                      conditional_guidance_scale_temporal=None, mask=None, x0=None, guidance_rescale=0.0, **kwargs):
+                      conditional_guidance_scale_temporal=None, mask=None, x0=None, guidance_rescale=0.0,
+                      noise_generators=None, **kwargs):
         m = self.model
         b, device = x.shape[0], x.device
         if unconditional_conditioning is None or unconditional_guidance_scale == 1.0:
@@ -322,11 +340,11 @@ class DDIMSampler(object):
             if guidance_rescale > 0.0:
                 model_output = rescale_noise_cfg(model_output, e_c, guidance_rescale=guidance_rescale)
         return self._ddim_update(x, t, index, model_output, c, repeat_noise, use_original_steps, quantize_denoised,
-                                 temperature, noise_dropout, score_corrector, corrector_kwargs)
+                                 temperature, noise_dropout, score_corrector, corrector_kwargs, noise_generators)
 
     def _ddim_update(self, x, t, index, model_output, c, repeat_noise, use_original_steps, quantize_denoised,
-                     temperature, noise_dropout, score_corrector, corrector_kwargs):
-        """ddim.py:231-277: v -> (eps, x0), dynamic rescale, x_{t-1}."""
+                     temperature, noise_dropout, score_corrector, corrector_kwargs, noise_generators=None):
+        """ddim.py:231-277: v -> (eps, x0), dynamic rescale, x_{t-1}; noise_generators: see sample()."""
         m = self.model
         b, device = x.shape[0], x.device
         e_t = m.predict_eps_from_z_and_v(x, t, model_output) if m.parameterization == "v" else model_output
@@ -350,9 +368,10 @@ class DDIMSampler(object):
             pred_x0, _, *_ = m.first_stage_model.quantize(pred_x0)
         dir_xt = (1.0 - a_prev - sigma_t ** 2).sqrt() * e_t
         if repeat_noise:
-            nz = torch.randn((1, *x.shape[1:]), device=device).repeat(b, *((1,) * (x.dim() - 1)))
+            gens = None if noise_generators is None else noise_generators[:1]
+            nz = randn_rows((1, *x.shape[1:]), device, gens).repeat(b, *((1,) * (x.dim() - 1)))
         else:
-            nz = torch.randn(x.shape, device=device)
+            nz = randn_rows(x.shape, device, noise_generators)
         noise = sigma_t * nz * temperature
         if noise_dropout > 0.0:
             noise = torch.nn.functional.dropout(noise, p=noise_dropout)
@@ -385,7 +404,7 @@ class DDIMSamplerMultiCond(DDIMSampler):
     def p_sample_ddim(self, x, c, t, index, repeat_noise=False, use_original_steps=False, quantize_denoised=False,
                       temperature=1.0, noise_dropout=0.0, score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1.0, unconditional_conditioning=None, uc_type=None, cfg_img=None,
-                      mask=None, x0=None, guidance_rescale=0.0, **kwargs):
+                      mask=None, x0=None, guidance_rescale=0.0, noise_generators=None, **kwargs):
         m = self.model
         cfg_img = unconditional_guidance_scale if cfg_img is None else cfg_img
         uc_img = kwargs["unconditional_conditioning_img_nonetext"]
@@ -399,4 +418,4 @@ class DDIMSamplerMultiCond(DDIMSampler):
             if guidance_rescale > 0.0:
                 model_output = rescale_noise_cfg(model_output, e_c, guidance_rescale=guidance_rescale)
         return self._ddim_update(x, t, index, model_output, c, repeat_noise, use_original_steps, quantize_denoised,
-                                 temperature, noise_dropout, score_corrector, corrector_kwargs)
+                                 temperature, noise_dropout, score_corrector, corrector_kwargs, noise_generators)

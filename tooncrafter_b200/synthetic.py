@@ -48,6 +48,26 @@ def fill_module_(module: torch.nn.Module, seed: int = 0, prefix: str = "") -> No
             p.copy_(synthetic_tensor(prefix + k, tuple(p.shape), seed).to(p.dtype))
 
 
+def synthetic_model(config, device, seed: int = 0) -> torch.nn.Module:
+    """instantiate_from_config(config) with the weights fill_module_(model, seed) gives, built straight on `device`
+    (meta skeleton, each tensor drawn on the host and copied over), so a full-size model needs no host-side copy."""
+    from . import diffusion, modules
+    with torch.device("meta"):
+        skeleton = diffusion.instantiate_from_config(config)
+    m = skeleton.to_empty(device=device)
+    m.reset_schedule_buffers()
+    with torch.no_grad():
+        for k, p in m.named_parameters():
+            p.copy_(synthetic_tensor(k, tuple(p.shape), seed).to(p.dtype))
+        for mod in m.modules():                 # constructor-made buffers that to_empty() left uninitialised
+            if isinstance(mod, modules.FrozenOpenCLIPEmbedder):
+                mod.model.attn_mask.fill_(float("-inf")).triu_(1)
+            elif isinstance(mod, modules.FrozenOpenCLIPImageEmbedderV2):
+                mod.mean.copy_(torch.tensor(modules.CLIP_MEAN))
+                mod.std.copy_(torch.tensor(modules.CLIP_STD))
+    return m.eval()
+
+
 def synthetic_inputs(B: int, T: int, h: int, w: int, context_dim: int = 1024, seed: int = 123,
                      latent_channels: int = 4):
     """x_T, cond / uncond dicts in the shapes scripts/evaluation/inference.py:189-216 builds."""
