@@ -66,15 +66,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (-> cudaErrorLaunchFailure) instead of hanging the GPU.  No printf here: the MMA
+// warpgroups wait inside their wgmma k-loop, and any function call there (printf, assert) makes ptxas serialise every
+// wgmma.mma_async of the kernel (warning C7510).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try_wait(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try_wait(bar, parity)) {
-        if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-            printf("tc: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-            __trap();
-        }
+        if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
     }
 }
 
@@ -114,20 +113,63 @@ template <int kN>
 __device__ __forceinline__ void wgmma_wait() {
     asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kN) : "memory");
 }
-// D[64 x 32] += A[64 x 16] * B[16 x 32]: fp16 operands, both K-major in shared memory; this thread's 16 accumulators
-// (row = 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column = 8 * (i >> 2) + 2 * (lane % 4) + (i & 1))
-__device__ __forceinline__ void wgmma_m64n32k16(float (&d)[16], uint64_t desc_a, uint64_t desc_b) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, 0, 0;\n\t"
-        "}\n"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(desc_a), "l"(desc_b));
-}
+// D[64 x N] += A[64 x 16] * B[16 x N], N = 32 kNJ: fp16 operands, both K-major in shared memory; this thread's 16 kNJ
+// accumulators (row = 16 * warp + lane / 4 + 8 * ((i >> 1) & 1), column = 8 * (i >> 2) + 2 * (lane % 4) + (i & 1)).
+// One instruction per k16 step reads A once for all N columns.  The operand lists are spelled out by the macros below
+// (asm templates are string literals); operands 0 .. 16 kNJ - 1 are the accumulators, then the two descriptors.
+template <int kNJ>
+__device__ __forceinline__ void wgmma_m64nNk16(float (&d)[16 * kNJ], uint64_t desc_a, uint64_t desc_b);
+
+#define TC_WG_R16_0 "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+#define TC_WG_R16_1 "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define TC_WG_R16_2 "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+#define TC_WG_R16_3 "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define TC_WG_R16_4 "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+#define TC_WG_R16_5 "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define TC_WG_R16_6 "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+#define TC_WG_R16_7 "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+#define TC_WG_REGS_1 TC_WG_R16_0
+#define TC_WG_REGS_2 TC_WG_REGS_1 ", " TC_WG_R16_1
+#define TC_WG_REGS_3 TC_WG_REGS_2 ", " TC_WG_R16_2
+#define TC_WG_REGS_4 TC_WG_REGS_3 ", " TC_WG_R16_3
+#define TC_WG_REGS_5 TC_WG_REGS_4 ", " TC_WG_R16_4
+#define TC_WG_REGS_6 TC_WG_REGS_5 ", " TC_WG_R16_5
+#define TC_WG_REGS_7 TC_WG_REGS_6 ", " TC_WG_R16_6
+#define TC_WG_REGS_8 TC_WG_REGS_7 ", " TC_WG_R16_7
+#define TC_WG_ACC16(o)                                                                                                  \
+    "+f"(d[o + 0]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]),     \
+        "+f"(d[o + 7]), "+f"(d[o + 8]), "+f"(d[o + 9]), "+f"(d[o + 10]), "+f"(d[o + 11]), "+f"(d[o + 12]),              \
+        "+f"(d[o + 13]), "+f"(d[o + 14]), "+f"(d[o + 15])
+#define TC_WG_ACC_1 TC_WG_ACC16(0)
+#define TC_WG_ACC_2 TC_WG_ACC_1, TC_WG_ACC16(16)
+#define TC_WG_ACC_3 TC_WG_ACC_2, TC_WG_ACC16(32)
+#define TC_WG_ACC_4 TC_WG_ACC_3, TC_WG_ACC16(48)
+#define TC_WG_ACC_5 TC_WG_ACC_4, TC_WG_ACC16(64)
+#define TC_WG_ACC_6 TC_WG_ACC_5, TC_WG_ACC16(80)
+#define TC_WG_ACC_7 TC_WG_ACC_6, TC_WG_ACC16(96)
+#define TC_WG_ACC_8 TC_WG_ACC_7, TC_WG_ACC16(112)
+// NJ, N = 32 NJ, and the operand numbers of the two descriptors (16 NJ, 16 NJ + 1)
+#define TC_WGMMA_M64NK16(NJ, N, DA, DB)                                                                                 \
+    template <>                                                                                                         \
+    __device__ __forceinline__ void wgmma_m64nNk16<NJ>(float(&d)[16 * NJ], uint64_t desc_a, uint64_t desc_b) {          \
+        asm volatile("{\n\t"                                                                                            \
+                     ".reg .pred p;\n\t"                                                                                \
+                     "setp.ne.b32 p, 1, 0;\n\t"                                                                         \
+                     "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 "                                          \
+                     "{" TC_WG_REGS_##NJ "}, %" #DA ", %" #DB ", p, 1, 1, 0, 0;\n\t"                                    \
+                     "}\n"                                                                                              \
+                     : TC_WG_ACC_##NJ                                                                                   \
+                     : "l"(desc_a), "l"(desc_b));                                                                       \
+    }
+TC_WGMMA_M64NK16(1, 32, 16, 17)
+TC_WGMMA_M64NK16(2, 64, 32, 33)
+TC_WGMMA_M64NK16(3, 96, 48, 49)
+TC_WGMMA_M64NK16(4, 128, 64, 65)
+TC_WGMMA_M64NK16(5, 160, 80, 81)
+TC_WGMMA_M64NK16(6, 192, 96, 97)
+TC_WGMMA_M64NK16(7, 224, 112, 113)
+TC_WGMMA_M64NK16(8, 256, 128, 129)
+#undef TC_WGMMA_M64NK16
 
 // ---- programmatic dependent launch: every kernel of this library is launched with the programmatic-stream-serialization
 // attribute (tc_host::launch), lets its successor's CTAs start early (launch_dependents) and must execute pdl_wait()

@@ -7,13 +7,16 @@
 //                                  by coordinate offset; out-of-bounds rows/cols are zero-filled by TMA == padding) and
 //                                  one 2-D box of the [Cout][taps*C] weight matrix, both 128B-swizzled, into a ring of
 //                                  `stages` shared-memory slots guarded by full / empty mbarriers.
-//   warpgroups 1-2 wgmma         : each owns 64 of the tile's 128 rows; m64n32k16 instructions over BN/32 column chunks,
-//                                  fp32 accumulators in registers, one k-block in flight behind the one being issued.
-//                                  After the last k-block the accumulators go to shared memory (the drained operand
-//                                  ring is reused), and the same 256 threads run the epilogue with one output row per
-//                                  thread and two column groups: folded LayerNorm / bias / timestep embedding / scale /
-//                                  residual or GEGLU -> fp16 -> 16-byte stores; optional per-row {sum, sumsq} of the
-//                                  outputs for the consumer's LayerNorm fold.
+//   warpgroups 1-2 wgmma         : each owns 64 of the tile's 128 rows; one m64nNk16 instruction per k16 step with
+//                                  N = BNp (BN rounded up to 32), so A is read from shared memory once per step for all
+//                                  columns; fp32 accumulators in registers, one k-block in flight behind the one being
+//                                  issued.  The k-loop makes no function call (see tc::mbar_wait), which would make
+//                                  ptxas serialise the wgmmas.  After the last k-block the accumulators go to shared
+//                                  memory (the drained operand ring is reused as an fp32 staging tile), and the same
+//                                  256 threads run the epilogue with one output row per thread and two column groups:
+//                                  folded LayerNorm / bias / timestep embedding / scale / residual or GEGLU -> fp16 ->
+//                                  16-byte stores; optional per-row {sum, sumsq} of the outputs for the consumer's
+//                                  LayerNorm fold.
 //   split-K (few output tiles, long K loops): every slice parks its fp32 tile in a workspace, takes a ticket, and the
 //   last slice to arrive sums all slices in slice order (deterministic) and runs the epilogue.
 //
@@ -73,7 +76,7 @@ __device__ __forceinline__ uint32_t pack_h2(float x, float y) {
     return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// kNJ = BNp / 32: column chunks of one m64n32k16 accumulator each (BNp = BN rounded up to 32)
+// kNJ = BNp / 32 (BNp = BN rounded up to 32): the wgmma is m64n(32 kNJ)k16
 template <int kNJ>
 __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_constant__ GemmKParams p) {
     tc::pdl_launch_dependents();   // the successor's prologue may overlap this kernel; it blocks in its own pdl_wait
@@ -152,11 +155,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
         s_bias[et] = (ok && p.bias) ? __ldg(p.bias + col) : 0.f;
         s_u[et] = (ok && p.ln_u) ? __ldg(p.ln_u + col) : 0.f;
     }
-    float acc[kNJ][16];
+    float acc[16 * kNJ];   // element 16 j + i: column 32 j + 8 (i >> 2) + 2 (lane % 4) + (i & 1)
 #pragma unroll
-    for (int j = 0; j < kNJ; ++j)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) acc[j][i] = 0.f;
+    for (int i = 0; i < 16 * kNJ; ++i) acc[i] = 0.f;
     {
         const uint64_t a_desc0 = tc::wgmma_desc_sw128(tc::smem_u32(sA + wg * 64 * 128));
         const uint64_t b_desc0 = tc::wgmma_desc_sw128(tc::smem_u32(sB));
@@ -168,11 +169,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
             const uint64_t ad = a_desc0 + (uint64_t)(stage * (kAStageBytes >> 4));
             const uint64_t bd = b_desc0 + (uint64_t)(stage * (p.b_bytes >> 4));
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k) {
-#pragma unroll
-                for (int j = 0; j < kNJ; ++j)   // chunk j: B rows [32 j, 32 j + 32) = +4096 bytes
-                    tc::wgmma_m64n32k16(acc[j], ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k + 256 * j));
-            }
+            for (int k = 0; k < kBlockK / 16; ++k)   // +32 bytes along the swizzled K row per k16 step
+                tc::wgmma_m64nNk16<kNJ>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k));
             tc::wgmma_commit();
             tc::wgmma_wait<1>();              // the previous k-block's MMAs have finished reading their slot
             if (prev >= 0) {
@@ -194,7 +192,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
             for (int i = 0; i < 16; i += 2) {
                 const int r = r0 + 8 * ((i >> 1) & 1);
                 const int c = j * 32 + 8 * (i >> 2) + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(stg + r * kLds + c) = make_float2(acc[j][i], acc[j][i + 1]);
+                *reinterpret_cast<float2*>(stg + r * kLds + c) = make_float2(acc[16 * j + i], acc[16 * j + i + 1]);
             }
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -364,9 +362,13 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
 // Tile-shape heuristic: pick (block_n, k-slices) minimising   waves x per-tile cycles   with a small model of one
 // k-block (M128 x bn x K64): tensor time at the data-sheet dense fp16 rate (989 TFLOP/s over 132 SMs: ~4 bn cycles), or
 // the ingest of its operands (A 16 KB + B bn x 128 B) at an assumed 52 B/clk/SM from L2, plus an assumed ~1500 cycles of
-// per-tile pipeline fill / epilogue tail.  The ingest rate, the per-tile overhead and the split-K overhead below are model
-// parameters, not measured on the H100.  Matters for
-// the 10x16 and 5x8 UNet levels (M = 5120 / 1280 rows), where one wave of 256-wide tiles leaves most SMs idle.
+// per-tile pipeline fill / epilogue tail.  Matters for the 10x16 and 5x8 UNet levels (M = 5120 / 1280 rows), where one
+// wave of 256-wide tiles leaves most SMs idle.
+// Checked against per-shape sweeps of the full-width-wgmma kernel (scripts/bench_gemm.py --sweep) on the 15 largest
+// shapes of a clip: 14 choices are within 5 % of the best measured (block_n, k-slices).  Known miss: the split-K term is
+// too small for 5120 x 1280 at K = 11520 (3x3 conv), which splits where one 256-wide slice is ~20 % faster; a larger term
+// stops 5120 x 640 at K = 5760 from splitting, which the model must keep, so a single constant cannot fit both.  The
+// tensor rate, the 52 B/clk ingest and the per-tile overhead are the original estimates, not fitted.
 struct TileChoice {
     int bn;
     int ksplit;
