@@ -55,6 +55,9 @@ int tc_sm_count(void);
  * autoencoder_dualref.py:52-69,914-935), nn.Conv3d (3,1,1) (openaimodel3d.py:255-266; autoencoder_dualref.py
  * :601-648), nn.Linear (attention.py:53-57,269,290,336,362,418,438), nn.Conv1d k=1 (attention.py:332-334,360).
  * C must be a multiple of 64 (callers zero-pad 4/8/3-channel inputs).
+ * Refused with TC_ERR_INVALID (nothing is launched): a, b, out, res or bias2 not 16-byte aligned; A strides, ldb, ldc,
+ * ldr or bias2_ld not multiples of 8 elements; n_cols > b_rows; ldc < the output width; ldr < n_cols with a residual;
+ * GEGLU with res, bias2, acc_scale != 1 or n_cols % block_n != 0.
  */
 typedef struct {
   /* A operand: [a_N][a_H][a_W][C] halfs, C contiguous, strides in elements */

@@ -44,6 +44,7 @@ def conv_gemm(a, a_dims, a_strides, w, taps, out, out_dims, n_cols, *, ldc=None,
     X = torch.cat(cols, dim=-1).reshape(M, len(taps) * C)
     assert w.shape[1] == len(taps) * C, f"weight K {w.shape[1]} != taps*C {len(taps) * C}"
     assert n_cols <= w.shape[0]
+    assert not geglu or acc_scale == 1.0, "GEGLU takes no acc_scale"
     acc = X @ w[:n_cols].float().t()
     if ln_stats is not None and ln_nslots > 0:
         # partial {sum, sumsq} slots written by a producer launch (any slot layout: only the totals matter)
@@ -74,11 +75,11 @@ def conv_gemm(a, a_dims, a_strides, w, taps, out, out_dims, n_cols, *, ldc=None,
     _view2d(out, M, width, ldc, out_offset).copy_(val.half())
     if row_stats is not None:
         assert block_n > 0 and row_stats_slots == -(-n_cols // block_n) and not geglu
-        q = val.half().float()
+        # slot j / block_n: the fp16-rounded outputs of one N tile
+        q = F.pad(val.half().float(), (0, row_stats_slots * block_n - n_cols)).view(M, row_stats_slots, block_n)
         rs = row_stats.view(-1)[:M * row_stats_slots * 2].view(M, row_stats_slots, 2)
-        rs.zero_()
-        rs[:, 0, 0] = q.sum(1)
-        rs[:, 0, 1] = (q * q).sum(1)
+        rs[:, :, 0] = q.sum(2)
+        rs[:, :, 1] = (q * q).sum(2)
 
 
 def groupnorm(x, y, gamma, beta, *, frames, frames_per_stat, hw, C, G=32, eps=1e-5, silu=False, ldx=None, ldy=None,

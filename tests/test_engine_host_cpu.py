@@ -94,8 +94,15 @@ def _check_conv_gemm_call(a, kw):
     if geglu:
         bn = kw.get("block_n", 0)
         assert bn > 0 and bn % 64 == 0 and n_cols % bn == 0 and kw.get("res") is None and kw.get("bias2") is None
+        assert kw.get("acc_scale", 1.0) == 1.0, "GEGLU takes no acc_scale"
     if kw.get("res") is not None:
-        assert (kw.get("ldr") or n_cols) % 8 == 0
+        ldr = kw.get("ldr") or n_cols
+        assert ldr % 8 == 0 and ldr >= n_cols
+    b2 = kw.get("bias2")
+    if b2 is not None:
+        # read 8 halfs (16 bytes) at a time: aligned base, row stride a multiple of 8
+        assert b2.dtype == torch.float16 and b2.stride(0) % 8 == 0 and b2.storage_offset() % 8 == 0
+        assert b2.shape[1] >= n_cols and kw.get("bias2_rows_per", 0) > 0
     if kw.get("ln_stats") is not None:
         assert kw.get("ln_u") is not None and n_cols % 16 == 0
         if kw.get("ln_nslots", 0):

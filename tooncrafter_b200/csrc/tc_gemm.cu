@@ -461,13 +461,20 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
                  "tc_conv_gemm: row_stats needs an explicit block_n and row_stats_slots == ceil(n_cols/block_n)");
     TC_CHECK_ARG(!d->res || (d->ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(d->res) & 15) == 0),
                  "tc_conv_gemm: residual must be 16-byte aligned");
+    TC_CHECK_ARG(!d->res || d->ldr >= d->n_cols, "tc_conv_gemm: ldr must be >= n_cols");
+    // the epilogue reads bias2 8 halfs (16 bytes) at a time
+    TC_CHECK_ARG(!d->bias2 || (d->bias2_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(d->bias2) & 15) == 0),
+                 "tc_conv_gemm: bias2 must be 16-byte aligned with bias2_ld % 8 == 0");
+    TC_CHECK_ARG(d->n_cols <= d->b_rows, "tc_conv_gemm: n_cols must be <= b_rows");
     const bool geglu = (d->flags & TC_EPI_GEGLU) != 0;
+    TC_CHECK_ARG(d->ldc >= (geglu ? d->n_cols / 2 : d->n_cols), "tc_conv_gemm: ldc must be >= the output width");
     int BN = d->block_n > 0 ? d->block_n : 0;   // 0: chosen below, once the M tiling is known
     TC_CHECK_ARG(BN == 0 || (BN % 16 == 0 && BN >= 16 && BN <= 256),
                  "tc_conv_gemm: block_n must be a multiple of 16 in [16,256]");
     if (geglu) {
         TC_CHECK_ARG(BN > 0 && BN % 32 == 0 && d->n_cols % BN == 0, "tc_conv_gemm: GEGLU needs n_cols % block_n == 0");
         TC_CHECK_ARG(!d->res && !d->bias2, "tc_conv_gemm: GEGLU epilogue takes bias only");
+        TC_CHECK_ARG(d->acc_scale == 1.0f, "tc_conv_gemm: GEGLU epilogue takes no acc_scale");
     }
 
     GemmKParams p;
