@@ -127,16 +127,19 @@ int tc_debug_read_attn_trace(unsigned long long* host_dst, int count);
  *                                                                       autoencoder_dualref.py:601,626)
  * Output may be written into a channel slice of a wider tensor (ldy >= C); input likewise (ldx).
  * `ws` needs 2*n_stat*G*TC_GN_MAX_PARTIALS floats (n_stat = frames/frames_per_stat).
+ * Refused (TC_ERR_INVALID, nothing launched): x or y not 16-byte aligned, ldx or ldy not a multiple of 8 or below C.
  */
 int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy, const float* gamma, const float* beta,
                  int frames, int frames_per_stat, int hw, int C, int G, float eps, int silu, float* ws,
                  void* stream);
 
 /* per-row {mean, rstd} of [rows][C] halfs (the statistics half of nn.LayerNorm, attention.py:225-227); the
- * normalisation itself is folded into the consuming tc_conv_gemm (ln_stats / ln_u). */
+ * normalisation itself is folded into the consuming tc_conv_gemm (ln_stats / ln_u).
+ * Refused: x not 16-byte or stats not 8-byte aligned, ldx not a multiple of 8 or below C. */
 int tc_row_stats(const void* x, long long ldx, int rows, int C, float eps, float* stats, void* stream);
 
-/* LayerNorm over the last dim of [rows][C] halfs (attention.py:225-227), fp32 math, fp16 out. */
+/* LayerNorm over the last dim of [rows][C] halfs (attention.py:225-227), fp32 math, fp16 out.
+ * Refused: x or y not 16-byte aligned, ldx or ldy not a multiple of 8 or below C. */
 int tc_layernorm(const void* x, long long ldx, void* y, long long ldy, const float* gamma, const float* beta,
                  int rows, int C, float eps, void* stream);
 
@@ -161,7 +164,8 @@ typedef struct {
 int tc_attention(const TcAttention* desc, void* stream);
 
 /* Temporal self-attention over the frame axis (attention.py:365-412 'only_self_att', einsum path :103-120):
- * tokens x[b][t][p][heads*64]; for each (b, p, head) softmax(q k^T * scale) v over t in [0,T), T <= 32. */
+ * tokens x[b][t][p][heads*64]; for each (b, p, head) softmax(q k^T * scale) v over t in [0,T), T <= 32.
+ * Refused: q, k, v or out not 16-byte aligned, ld or ldo not a multiple of 8 or below heads*64. */
 int tc_temporal_attention(const void* q, const void* k, const void* v, long long ld, void* out, long long ldo,
                           int B, int T, int P, int heads, float scale, void* stream);
 
@@ -173,7 +177,7 @@ int tc_attention_wide(const void* q, const void* k, const void* v, long long ldq
                       void* out, long long ldo, int batches, int Lq, int Lk, int D, float scale, void* stream);
 
 /* row softmax of fp16 scores [rows][cols] scaled by `scale`, in place (unfused form of the VAE mid-block attention, d = 512:
- * autoencoder_dualref.py:172-200) */
+ * autoencoder_dualref.py:172-200).  Any sign of `scale`: the maximum is taken over the scaled scores.  Refused: lds < cols. */
 int tc_softmax_rows(void* s, long long lds, int rows, int cols, float scale, void* stream);
 
 /* ------------------------------------------------------------------------------------------------

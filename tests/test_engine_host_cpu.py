@@ -113,6 +113,51 @@ def _check_conv_gemm_call(a, kw):
         assert kw["row_stats"].numel() >= 2 * kw["row_stats_slots"] * out_dims[0] * out_dims[1] * out_dims[2]
 
 
+def _aligned(t, off=0):
+    """16-byte aligned operand: the tensor's element offset plus the op's offset is a multiple of 8 halfs."""
+    return (t.storage_offset() + off) % 8 == 0
+
+
+def _check_norm_attention_call(fn, a, kw):
+    """Preconditions tc_groupnorm, tc_layernorm, tc_row_stats, tc_temporal_attention and tc_attention enforce
+    (include/tooncrafter_b200.h, TC_CHECK_ARG in csrc/tc_norm.cu and csrc/tc_attn.cu)."""
+    from tooncrafter_b200 import ops
+    name = fn.__name__
+    if fn in (ops.groupnorm, ops.layernorm, ops.row_stats):
+        C = kw["C"]
+        ldx = kw.get("ldx") or C
+        assert C % 8 == 0 and ldx % 8 == 0 and ldx >= C and _aligned(a[0], kw.get("x_offset", 0)), name
+        if fn is ops.row_stats:
+            assert a[1].storage_offset() % 2 == 0, "row_stats: 8-byte aligned statistics"
+        else:
+            ldy = kw.get("ldy") or C
+            assert ldy % 8 == 0 and ldy >= C and _aligned(a[1], kw.get("y_offset", 0)), name
+    elif fn is ops.temporal_attention:
+        C = kw["heads"] * 64
+        assert kw["ld"] % 8 == 0 and kw["ldo"] % 8 == 0 and kw["ld"] >= C and kw["ldo"] >= C and 0 < kw["T"] <= 32
+        for t, off in zip(a, ("q_offset", "k_offset", "v_offset", None)):
+            assert _aligned(t, kw.get(off, 0) if off else 0), f"temporal_attention: {off or 'out'} misaligned"
+    elif fn is ops.attention:
+        q, segs, out = a
+        assert kw["ldq"] % 8 == 0 and kw["ldo"] % 8 == 0 and 1 <= len(segs) <= 2
+        assert _aligned(q, kw.get("q_offset", 0)) and _aligned(out, kw.get("out_offset", 0))
+        for sg in segs:
+            assert sg["ldk"] % 8 == 0 and sg["ldv"] % 8 == 0 and sg["Lk"] > 0 and sg.get("kv_div", 1) > 0
+            assert _aligned(sg["k"], sg.get("k_offset", 0)) and _aligned(sg["v"], sg.get("v_offset", 0))
+
+
+def _check_program(calls):
+    from tooncrafter_b200 import ops
+    seen = set()
+    for fn, a, kw in calls:
+        if fn is ops.conv_gemm:
+            _check_conv_gemm_call(a, kw)
+        elif fn in (ops.groupnorm, ops.layernorm, ops.row_stats, ops.temporal_attention, ops.attention):
+            _check_norm_attention_call(fn, a, kw)
+            seen.add(fn.__name__)
+    return seen
+
+
 def test_programs_plan_for_other_geometries_with_valid_launch_arguments():
     """Planning is pure host logic: build the full-size UNet / VAE programs on the meta device for the 512 and the 1024
     model geometry (configs/training_1024_v1.0: latent 72x128) and a small odd one, and check every recorded tc_conv_gemm
@@ -128,16 +173,13 @@ def test_programs_plan_for_other_geometries_with_valid_launch_arguments():
         calls = list(plan.ctx.calls) + list(plan.main.calls)
         gemms = [(a, kw) for fn, a, kw in calls if fn is ops.conv_gemm]
         assert len(plan.main) == 664 and len(gemms) > 400
-        for a, kw in gemms:
-            _check_conv_gemm_call(a, kw)
+        assert _check_program(calls) == {"groupnorm", "attention", "temporal_attention"}
         assert plan.arena.high_water < (170 << 30)
     deng = vae_engine.DecoderEngine(dec, device="meta", plan_only=True)
     for (T, h, w) in ((16, 40, 64), (14, 40, 64), (16, 72, 128)):
         plan = deng.plan_for(T, h, w)
         calls = list(plan.ctx.calls) + list(plan.main.calls)
-        for fn, a, kw in calls:
-            if fn is ops.conv_gemm:
-                _check_conv_gemm_call(a, kw)
+        assert _check_program(calls) == {"groupnorm", "attention"}
         assert plan.arena.high_water < (170 << 30)
         # the mid-block AttnBlock (autoencoder_dualref.py:172-206) is ONE fused launch: head dim = its 512 channels, q / k / v
         # channel slices of one projection output, no score matrix in memory (no softmax_rows, no per-frame score GEMMs)
@@ -182,3 +224,14 @@ def test_engine_repacks_when_any_parameter_changes():
     with torch.no_grad():
         list(m.parameters())[-1].add_(1.0)
     assert not eng.matches(m)
+
+
+def test_openclip_programs_plan_with_valid_launch_arguments():
+    """The full-size OpenCLIP text and image tower programs, planned on the meta device: every tc_conv_gemm,
+    tc_layernorm, tc_row_stats and tc_attention call satisfies the C ABI's preconditions."""
+    from tooncrafter_b200.cond_engine import ClipImageEngine, ClipTextEngine
+    with torch.device("meta"):
+        t = modules.FrozenOpenCLIPEmbedder(layer="penultimate")
+        i = modules.FrozenOpenCLIPImageEmbedderV2()
+    for eng, B in ((ClipTextEngine(t, device="meta", plan_only=True), 2), (ClipImageEngine(i, device="meta", plan_only=True), 2)):
+        assert _check_program(list(eng.plan_for(B).main.calls)) == {"layernorm", "row_stats", "attention"}

@@ -550,7 +550,8 @@ def test_attention_wide(ops, N, L, D):
 
 
 def test_attention_wide_growing_maximum(ops):
-    """Keys whose scores grow along the sequence force the lazy O rescale (and its wait on the previous PV MMA)."""
+    """Keys whose scores grow along the sequence: later key tiles raise the row maximum, so the running output and
+    softmax sum are rescaled by exp2(m_old - m_new) on those tiles."""
     N, L, D = 2, 1024, 512
     qkv = _rand(N, L, 3 * D, seed=92)
     qkv[..., D:2 * D] *= torch.linspace(0.2, 3.0, L, device=DEV)[None, :, None]

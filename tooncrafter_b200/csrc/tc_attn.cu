@@ -514,8 +514,9 @@ __global__ void softmax_rows_kernel(__half* __restrict__ s, long long lds, int r
     __half* r = s + (long long)row * lds;
     __shared__ float red[32];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
+    // the maximum of the scaled scores: exp2(x * scale - m) <= 1 for either sign of the scale
     float m = -INFINITY;
-    for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, __half2float(r[c]));
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) m = fmaxf(m, __half2float(r[c]) * scale_log2);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if (lane == 0) red[warp] = m;
@@ -524,7 +525,7 @@ __global__ void softmax_rows_kernel(__half* __restrict__ s, long long lds, int r
     for (int w = 1; w < nw; ++w) m = fmaxf(m, red[w]);
     __syncthreads();
     float l = 0.f;
-    for (int c = threadIdx.x; c < cols; c += blockDim.x) l += exp2f((__half2float(r[c]) - m) * scale_log2);
+    for (int c = threadIdx.x; c < cols; c += blockDim.x) l += exp2f(__half2float(r[c]) * scale_log2 - m);
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
     if (lane == 0) red[warp] = l;
@@ -533,7 +534,7 @@ __global__ void softmax_rows_kernel(__half* __restrict__ s, long long lds, int r
     for (int w = 0; w < nw; ++w) l += red[w];
     const float inv = 1.0f / l;
     for (int c = threadIdx.x; c < cols; c += blockDim.x)
-        r[c] = __float2half_rn(exp2f((__half2float(r[c]) - m) * scale_log2) * inv);
+        r[c] = __float2half_rn(exp2f(__half2float(r[c]) * scale_log2 - m) * inv);
 }
 
 }  // namespace
@@ -554,10 +555,11 @@ static int launch_flash_kernel(const FaParams& p, dim3 grid, size_t smem_bytes, 
     return TC_OK;
 }
 
-// split_p: P as fp16 hi + lo parts for the PV product when few keys average its rounding (cross attention: 77 + 16 keys)
+// split_p: P as fp16 hi + lo parts for the PV product when few keys average its rounding (cross attention: 77 + 16 keys);
+// with the causal mask query i sees min(i + 1, Lk) keys, so no row sees more than Lq
 static int launch_flash(const FaParams& p0, int batches, int Lk_max, bool causal, cudaStream_t stream) {
     FaParams p = p0;
-    p.split_p = Lk_max <= 512 ? 1 : 0;
+    p.split_p = (causal && p.Lq < Lk_max ? p.Lq : Lk_max) <= 512 ? 1 : 0;
     // Q and K tiles of D halfs per row, V tile of DV halfs per row (80-wide rows padded to 11 chunks, tile_off)
     const size_t smem_bytes = (size_t)(tile_bytes(kFaRows, p.D) + tile_bytes(kFaKeys, p.D) + tile_bytes(kFaKeys, p.DV)) + 128;
     dim3 grid((p.Lq + kFaRows - 1) / kFaRows, p.heads * p.nv, batches);
@@ -671,6 +673,9 @@ extern "C" int tc_temporal_attention(const void* q, const void* k, const void* v
     TC_CHECK_ARG(q && k && v && out, "tc_temporal_attention: null pointer");
     TC_CHECK_ARG(B > 0 && T > 0 && T <= 32 && P > 0 && heads > 0, "tc_temporal_attention: need 0 < T <= 32");
     TC_CHECK_ARG(ld % 8 == 0 && ldo % 8 == 0, "tc_temporal_attention: strides must be multiples of 8");
+    TC_CHECK_ARG(ld >= 64LL * heads && ldo >= 64LL * heads, "tc_temporal_attention: ld and ldo must be at least heads * 64");
+    TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
+                   reinterpret_cast<uintptr_t>(out)) & 15) == 0, "tc_temporal_attention: operands must be 16-byte aligned");
     const long long items = (long long)B * P * heads;
     const float sl2 = scale * 1.4426950408889634f;
     const __half* qp = reinterpret_cast<const __half*>(q);
@@ -694,6 +699,7 @@ extern "C" int tc_temporal_attention(const void* q, const void* k, const void* v
 extern "C" int tc_softmax_rows(void* s, long long lds, int rows, int cols, float scale, void* stream_v) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
     TC_CHECK_ARG(s && rows > 0 && cols > 0, "tc_softmax_rows: bad arguments");
+    TC_CHECK_ARG(lds >= cols, "tc_softmax_rows: lds must be at least cols");
     tc_host::launch(softmax_rows_kernel, dim3(rows), dim3(256), 0, stream, 1, reinterpret_cast<__half*>(s), lds, rows, cols,
                                                   scale * 1.4426950408889634f);
     count_launch();

@@ -37,15 +37,15 @@ __device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
 }
 
 // ---- pass 1: per-block partial (sum, sumsq) per group -------------------------------------------------
-// grid = (nblk, n_stat); block = V * k threads (V = C/8), thread t owns channel vector t % V.
+// grid = (nblk, n_stat); block = V * rows_per_iter threads (V = C/8) rounded up to whole warps: thread t < V *
+// rows_per_iter owns channel vector t % V of pixel row t / V, the threads past them only take part in the reduction.
 __global__ void gn_stats_kernel(const __half* __restrict__ x, long long ldx, long long pixels_per_stat, int C, int G,
-                                float* __restrict__ partials) {
+                                int rows_per_iter, float* __restrict__ partials) {
     tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
     extern __shared__ float sm[];  // [rows_per_iter][2*C]: per-thread partials, reduced in a fixed order (deterministic)
     const int V = C >> 3;
     const int v = threadIdx.x % V;
     const int prow = threadIdx.x / V;
-    const int rows_per_iter = blockDim.x / V;
     const int s = blockIdx.y;
 
     float sum[8], sq[8];
@@ -54,7 +54,8 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, long long ldx, lon
     const __half* base = x + (long long)s * pixels_per_stat * ldx + (long long)v * 8;
     const long long stride = (long long)gridDim.x * rows_per_iter;
     // 4 independent 16-byte loads in flight per thread (the pass is pure HBM/L2 streaming)
-    for (long long pix = (long long)blockIdx.x * rows_per_iter + prow; pix < pixels_per_stat; pix += 4 * stride) {
+    const long long pix_end = prow < rows_per_iter ? pixels_per_stat : 0;
+    for (long long pix = (long long)blockIdx.x * rows_per_iter + prow; pix < pix_end; pix += 4 * stride) {
         uint4 u[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
@@ -74,15 +75,17 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, long long ldx, lon
             }
         }
     }
-    float* mine = sm + (long long)prow * 2 * C;
+    if (prow < rows_per_iter) {
+        float* mine = sm + (long long)prow * 2 * C;
 #pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        mine[v * 8 + i] = sum[i];
-        mine[C + v * 8 + i] = sq[i];
+        for (int i = 0; i < 8; ++i) {
+            mine[v * 8 + i] = sum[i];
+            mine[C + v * 8 + i] = sq[i];
+        }
     }
     __syncthreads();
     // block reduction in a fixed order (deterministic), one warp per (group, sum | sumsq) task rather than 32 threads
-    // walking rows_per_iter x cpg values serially
+    // walking rows_per_iter x cpg values serially (blockDim.x is a multiple of 32: every warp is whole)
     const int cpg = C / G;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
     const int n = rows_per_iter * cpg;
@@ -98,10 +101,10 @@ __global__ void gn_stats_kernel(const __half* __restrict__ x, long long ldx, lon
 }
 
 // ---- pass 2: finalize statistics for this block's stat group, then normalise (+SiLU) -------------------
-// grid = (blocks_per_stat, n_stat)
+// grid = (blocks_per_stat, n_stat); block as gn_stats_kernel (whole warps, V * rows_per_iter of them normalise)
 __global__ void gn_apply_kernel(const __half* __restrict__ x, long long ldx, __half* __restrict__ y, long long ldy,
                                 const float* __restrict__ gamma, const float* __restrict__ beta,
-                                long long pixels_per_stat, int C, int G, float eps, int silu,
+                                long long pixels_per_stat, int C, int G, int rows_per_iter, float eps, int silu,
                                 const float* __restrict__ partials, int nblk) {
     tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
     extern __shared__ float sm[];  // mean[G], rstd[G]
@@ -138,7 +141,7 @@ __global__ void gn_apply_kernel(const __half* __restrict__ x, long long ldx, __h
     const int V = C >> 3;
     const int v = threadIdx.x % V;
     const int prow = threadIdx.x / V;
-    const int rows_per_iter = blockDim.x / V;
+    if (prow >= rows_per_iter) return;
     float sc[8], sh[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -223,6 +226,10 @@ __global__ void __launch_bounds__(640, 1) gn_fused_kernel(const __half* __restri
 
     uint4 u[kMaxV];
     float sum = 0.f, sq = 0.f;
+    // sums are taken about a pivot, the unit's first element (the same for every CTA of the cluster): E[x^2] - E[x]^2
+    // from fp32 sums of raw values cancels when the mean is large against the spread, sums about a value within a few
+    // standard deviations of the mean do not
+    const float pivot = __half2float(x[(long long)s * pixels_per_stat * ldx + (long long)g * cpg]);
 #pragma unroll
     for (int i = 0; i < kMaxV; ++i) {
         const long long v = v_begin + threadIdx.x + (long long)i * T;
@@ -236,8 +243,9 @@ __global__ void __launch_bounds__(640, 1) gn_fused_kernel(const __half* __restri
             unpack8(u[i], f);
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-                sum += f[j];
-                sq += f[j] * f[j];
+                const float d = f[j] - pivot;
+                sum += d;
+                sq += d * d;
             }
         }
     }
@@ -274,10 +282,10 @@ __global__ void __launch_bounds__(640, 1) gn_fused_kernel(const __half* __restri
             b = s_cta[1];
         }
         const double cnt = (double)pixels_per_stat * (double)cpg;
-        const double mean = a / cnt;
-        double var = b / cnt - mean * mean;
+        const double dmean = a / cnt;                  // mean - pivot
+        double var = b / cnt - dmean * dmean;
         if (var < 0.0) var = 0.0;
-        s_stat[0] = (float)mean;
+        s_stat[0] = (float)((double)pivot + dmean);
         s_stat[1] = (float)(1.0 / sqrt(var + (double)eps));
     }
     __syncthreads();
@@ -414,6 +422,9 @@ extern "C" int tc_row_stats(const void* x, long long ldx, int rows, int C, float
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
     TC_CHECK_ARG(x && stats, "tc_row_stats: null pointer");
     TC_CHECK_ARG(C > 0 && C % 8 == 0 && C <= 2048 && ldx % 8 == 0 && rows > 0, "tc_row_stats: bad shape");
+    TC_CHECK_ARG(ldx >= C, "tc_row_stats: ldx must be at least C");
+    TC_CHECK_ARG((reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(stats) & 7) == 0,
+                 "tc_row_stats: x must be 16-byte and stats 8-byte aligned");
     const int threads = 256;
     const int blocks = (rows + 7) / 8;
     const __half* xp = reinterpret_cast<const __half*>(x);
@@ -440,6 +451,9 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
     TC_CHECK_ARG(frames > 0 && frames_per_stat > 0 && frames % frames_per_stat == 0 && hw > 0,
                  "tc_groupnorm: bad frame counts");
     TC_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0, "tc_groupnorm: strides must be multiples of 8");
+    TC_CHECK_ARG(ldx >= C && ldy >= C, "tc_groupnorm: ldx and ldy must be at least C");
+    TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0,
+                 "tc_groupnorm: x and y must be 16-byte aligned");
     const int n_stat = frames / frames_per_stat;
     const long long pps = (long long)frames_per_stat * hw;
     {
@@ -483,7 +497,9 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
     const int V = C / 8;
     int k = 512 / V;
     if (k < 1) k = 1;
-    const int threads = V * k;
+    // k pixel rows of V vectors per block, rounded up to whole warps (the warp-per-task reductions shuffle over all 32
+    // lanes); the surplus threads load nothing
+    const int threads = (V * k + 31) / 32 * 32;
     // small tensors are latency-bound (a chain of dependent load rounds per thread): spread them over as many blocks as
     // one round of 4 loads per thread allows; large ones are capped to one resident wave below
     long long want = (pps + (long long)k * 4 - 1) / ((long long)k * 4);
@@ -494,7 +510,7 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
     if (cap > kGnMaxPartials) cap = kGnMaxPartials;
     if (nblk > cap) nblk = cap;
     tc_host::launch(gn_stats_kernel, dim3(dim3(nblk, n_stat)), dim3(threads), (size_t)k * 2 * C * sizeof(float), stream, 1, 
-        reinterpret_cast<const __half*>(x), ldx, pps, C, G, ws);
+        reinterpret_cast<const __half*>(x), ldx, pps, C, G, k, ws);
     count_launch();
     TC_CHECK_LAUNCH("gn_stats_kernel");
     long long want2 = (pps + (long long)k * 4 - 1) / ((long long)k * 4);
@@ -504,7 +520,7 @@ extern "C" int tc_groupnorm(const void* x, long long ldx, void* y, long long ldy
     if (cap2 < 1) cap2 = 1;
     if (nblk2 > cap2) nblk2 = cap2;
     tc_host::launch(gn_apply_kernel, dim3(dim3(nblk2, n_stat)), dim3(threads), 2 * G * sizeof(float), stream, 1, 
-        reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, gamma, beta, pps, C, G, eps, silu,
+        reinterpret_cast<const __half*>(x), ldx, reinterpret_cast<__half*>(y), ldy, gamma, beta, pps, C, G, k, eps, silu,
         ws, nblk);
     count_launch();
     TC_CHECK_LAUNCH("gn_apply_kernel");
@@ -518,6 +534,9 @@ extern "C" int tc_layernorm(const void* x, long long ldx, void* y, long long ldy
     TC_CHECK_ARG(x && y && gamma && beta, "tc_layernorm: null pointer");
     TC_CHECK_ARG(C > 0 && C % 8 == 0 && C <= 2048, "tc_layernorm: need C % 8 == 0 and C <= 2048");
     TC_CHECK_ARG(ldx % 8 == 0 && ldy % 8 == 0 && rows > 0, "tc_layernorm: bad strides/rows");
+    TC_CHECK_ARG(ldx >= C && ldy >= C, "tc_layernorm: ldx and ldy must be at least C");
+    TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) & 15) == 0,
+                 "tc_layernorm: x and y must be 16-byte aligned");
     const int threads = 256;
     const int blocks = (rows + 7) / 8;
     const __half* xp = reinterpret_cast<const __half*>(x);
