@@ -235,3 +235,19 @@ def test_openclip_programs_plan_with_valid_launch_arguments():
         i = modules.FrozenOpenCLIPImageEmbedderV2()
     for eng, B in ((ClipTextEngine(t, device="meta", plan_only=True), 2), (ClipImageEngine(i, device="meta", plan_only=True), 2)):
         assert _check_program(list(eng.plan_for(B).main.calls)) == {"layernorm", "row_stats", "attention"}
+
+
+def test_plan_only_engines_refuse_to_execute_without_an_executor():
+    """A plan-only engine's programs hold CPU / meta tensors: without an executor to interpret them, executing raises
+    the engines' common error instead of reaching a launch."""
+    import pytest
+    from make_golden_clip import tiny_image, tiny_pixels, tiny_text, tiny_tokens
+    from make_golden_resampler import TINY, tiny_input
+    from tooncrafter_b200.cond_engine import ClipImageEngine, ClipTextEngine, ResamplerEngine
+    rs = modules.Resampler(**TINY).eval()
+    runs = [(ResamplerEngine(rs, device="cpu", plan_only=True), tiny_input()),
+            (ClipTextEngine(tiny_text(), device="cpu", plan_only=True), tiny_tokens()),
+            (ClipImageEngine(tiny_image(), device="cpu", plan_only=True), tiny_pixels())]
+    for eng, x in runs:
+        with pytest.raises(RuntimeError, match="plan_only engine cannot execute"):
+            eng.forward(x)

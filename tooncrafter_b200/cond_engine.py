@@ -10,25 +10,17 @@ on a few hundred tokens; it reuses the hot path's GEMM / LayerNorm / attention k
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import RowStats, _P, _f, _h, fold_layernorm, linear, ln_linear, pack_linear, weights_signature
-from .runtime import Act, Arena, Builder, Program
+from .engine import RowStats, _P, _f, _h, fold_layernorm, linear, ln_linear, pack_linear
+from .runtime import Act, Arena, Builder, Engine, Program
 
 
-class ResamplerEngine:
+class ResamplerEngine(Engine):
     def __init__(self, rs: nn.Module, device=None, use_graph: bool = False, plan_only: bool = False):
-        p0 = rs.latents
-        self.dev = torch.device(device) if device is not None else p0.device
-        self.plan_only = plan_only
-        if self.dev.type != "cuda" and not plan_only:
-            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
-        self._sig = weights_signature(rs)
-        self.use_graph = use_graph
+        super().__init__(rs, device, use_graph, plan_only)
         self.dim, self.heads, self.inner = rs.dim, rs.heads, rs.heads * rs.dim_head
         self.n_lat = rs.latents.shape[1]
         self.emb = rs.proj_in.weight.shape[1]
@@ -37,10 +29,6 @@ class ResamplerEngine:
             if n % 64:
                 raise NotImplementedError("Resampler widths must be multiples of 64 (GEMM K granularity)")
         self._pack(rs)
-        self._plans: Dict = {}
-
-    def matches(self, rs) -> bool:
-        return rs.latents.device == self.dev and self._sig == weights_signature(rs)
 
     def _pack(self, rs):
         dev = self.dev
@@ -111,21 +99,12 @@ class ResamplerEngine:
         ln(po.t, plan.out, self.p_out.norm, rows_l, self.out_dim)
         return plan
 
-    def plan_for(self, B: int, n1: int):
-        key = (B, n1)
-        if key not in self._plans:
-            self._plans[key] = self._build(B, n1)
-        return self._plans[key]
-
     def forward(self, x: torch.Tensor, executor=None) -> torch.Tensor:
         B, n1, E = x.shape
         assert E == self.emb, f"expected {self.emb}-wide image tokens"
         plan = self.plan_for(B, n1)
         plan.x_in.copy_(x.reshape(-1))
-        if executor is not None:
-            plan.main.run(executor)
-        else:
-            plan.main.replay(self.use_graph)
+        self._execute(plan.main, executor, self.use_graph)
         return plan.out.view(B, self.n_lat, self.out_dim).float()
 
 
@@ -134,7 +113,7 @@ CLIP_LN_EPS = 1e-5            # open_clip LayerNorm
 PATCH_K_PAD = 64              # GEMM K granularity: the 3 * patch^2 patch vector is zero-padded to a multiple of it
 
 
-class _ClipTowerEngine:
+class _ClipTowerEngine(Engine):
     """Shared part of the two OpenCLIP tower engines: the residual attention blocks of open_clip.transformer
     (reference condition.py:214-231, :369; open_clip ResidualAttentionBlock: x += attn(ln_1(x)); x += mlp(ln_2(x)),
     nn.MultiheadAttention with a fused in_proj, MLP c_fc -> GELU (erf) -> c_proj).
@@ -145,17 +124,8 @@ class _ClipTowerEngine:
     causal = False
 
     def __init__(self, m: nn.Module, device=None, use_graph: bool = False, plan_only: bool = False):
-        self.dev = torch.device(device) if device is not None else m.model.positional_embedding.device
-        self.plan_only = plan_only
-        if self.dev.type != "cuda" and not plan_only:
-            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
-        self._sig = weights_signature(m)
-        self.use_graph = use_graph
+        super().__init__(m, device, use_graph, plan_only)
         self.heads = m.heads
-        self._plans: Dict = {}
-
-    def matches(self, m) -> bool:
-        return m.model.positional_embedding.device == self.dev and self._sig == weights_signature(m)
 
     def _pack_blocks(self, blocks):
         dev = self.dev
@@ -209,12 +179,6 @@ class _ClipTowerEngine:
             x, st = x2, s2
         return x
 
-    def _run(self, plan, executor):
-        if executor is not None:
-            plan.main.run(executor)
-        else:
-            plan.main.replay(self.use_graph)
-
 
 class _LN:
     """LayerNorm view of an open_clip LayerNorm parameter pair (what fold_layernorm reads)."""
@@ -255,11 +219,6 @@ class ClipTextEngine(_ClipTowerEngine):
                ldx=W, ldy=W)
         return plan
 
-    def plan_for(self, B: int):
-        if B not in self._plans:
-            self._plans[B] = self._build(B)
-        return self._plans[B]
-
     def forward(self, tokens: torch.Tensor, executor=None) -> torch.Tensor:
         """tokens [B, ctx] int64 -> [B, ctx, width] fp32."""
         B, L = tokens.shape
@@ -267,7 +226,7 @@ class ClipTextEngine(_ClipTowerEngine):
         plan = self.plan_for(B)
         ids = tokens.to(self.dev)
         plan.x_in.view(B, L, self.width).copy_(self.tok[ids].float() + self.pos)
-        self._run(plan, executor)
+        self._execute(plan.main, executor, self.use_graph)
         return plan.out.view(B, L, self.width).float()
 
 
@@ -314,11 +273,6 @@ class ClipImageEngine(_ClipTowerEngine):
         self._blocks(bld, x, B, L, last_out=Act(plan.out, 1, 1, rows, W, W))
         return plan
 
-    def plan_for(self, B: int):
-        if B not in self._plans:
-            self._plans[B] = self._build(B)
-        return self._plans[B]
-
     def forward(self, pixels: torch.Tensor, executor=None) -> torch.Tensor:
         """pixels [B, 3, image, image] (CLIP-normalised) -> [B, 1 + grid^2, width] fp32."""
         B = pixels.shape[0]
@@ -328,5 +282,5 @@ class ClipImageEngine(_ClipTowerEngine):
         patches = pixels.to(self.dev).float().reshape(B, 3, g, P, g, P).permute(0, 2, 4, 1, 3, 5)
         xin = plan.x_in.view(B, self.n_tok, self.kpad)
         xin[:, 1:, :3 * P * P].copy_(patches.reshape(B, g * g, 3 * P * P))
-        self._run(plan, executor)
+        self._execute(plan.main, executor, self.use_graph)
         return plan.out.view(B, self.n_tok, self.width).float()

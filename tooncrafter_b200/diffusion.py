@@ -127,35 +127,29 @@ class AutoencoderKL(nn.Module):
         from . import runtime
         from .vae_engine import EncoderEngine
         ex = runtime.TEST_EXECUTOR
-        if self._enc_engine is None or not self._enc_engine.matches(self):
-            self._enc_engine = EncoderEngine(self, plan_only=ex is not None)
-        moments, hidden = self._enc_engine.encode(x, executor=ex)
+        moments, hidden = EncoderEngine.cached(self, "_enc_engine", ex).encode(x, executor=ex)
         post = DiagonalGaussianDistribution(moments)
         return (post, hidden) if return_hidden_states else post
 
     def decode(self, z, **kwargs):
         """kwargs: ref_context (5 maps [b, C, 2, H, W]) and timesteps, as decode_core passes them."""
-        from .vae_engine import DecoderEngine
         if len(kwargs) == 0:
             raise NotImplementedError("decode() without ref_context/timesteps never happens on the VideoDecoder path")
         from . import runtime
         ex = runtime.TEST_EXECUTOR
-        if self._dec_engine is None or not self._dec_engine.matches(self.decoder):
-            self._dec_engine = DecoderEngine(self.decoder, plan_only=ex is not None)
+        eng = self.decoder_engine()
         ref = kwargs.get("ref_context")
         T = kwargs.get("timesteps") or z.shape[0]
         if z.shape[0] != T:
             raise NotImplementedError("one clip per decode call (the reference mixes clips for B > 1)")
-        return self._dec_engine.decode(z.float(), ref, executor=ex).clone()
+        return eng.decode(z.float(), ref, executor=ex).clone()
 
     def decoder_engine(self):
         """The DecoderEngine decode() runs on (built on first use).  Its decode() returns a view of the plan's static
         output buffer, valid until the next decode of the same T: for callers that consume it in place."""
         from . import runtime
         from .vae_engine import DecoderEngine
-        if self._dec_engine is None or not self._dec_engine.matches(self.decoder):
-            self._dec_engine = DecoderEngine(self.decoder, plan_only=runtime.TEST_EXECUTOR is not None)
-        return self._dec_engine
+        return DecoderEngine.cached(self, "_dec_engine", runtime.TEST_EXECUTOR, module=self.decoder)
 
 
 class AutoencoderKL_Dualref(AutoencoderKL):

@@ -16,16 +16,14 @@ H100-first departures (results identical up to fp16 rounding):
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
-
-import os
+from typing import Optional
 
 import torch
 import torch.nn as nn
 
 from . import ops
 from .layout import Layer, UNetLayout
-from .runtime import Act, Arena, Builder, Program
+from .runtime import Act, Arena, Builder, Engine, Program
 
 GEGLU_BN = 256
 
@@ -91,16 +89,16 @@ def pack_transformer_block(tb, dev, cross: bool):
     """LayerNorms are folded into the GEMM that consumes them (fold_layernorm); q/k/v projections fused."""
     inner = tb.attn1.to_q.weight.shape[0]
     p = _P(inner=inner)
-    a1, a2 = tb.attn1, tb.attn2
-    p.qkv1 = fold_layernorm(torch.cat([a1.to_q.weight, a1.to_k.weight, a1.to_v.weight], 0), None, tb.norm1, dev)
-    p.o1_w, p.o1_b = pack_linear(a1.to_out[0].weight, dev), _f(a1.to_out[0].bias, dev)
+
+    def attn(a, norm, qkv: bool):
+        w = torch.cat([a.to_q.weight, a.to_k.weight, a.to_v.weight], 0) if qkv else a.to_q.weight
+        return _P(proj=fold_layernorm(w, None, norm, dev), o_w=pack_linear(a.to_out[0].weight, dev),
+                  o_b=_f(a.to_out[0].bias, dev))
+    a2 = tb.attn2
+    p.attn1, p.attn2 = attn(tb.attn1, tb.norm1, True), attn(a2, tb.norm2, not cross)
     if cross:
-        p.q2 = fold_layernorm(a2.to_q.weight, None, tb.norm2, dev)
         p.kv_txt = _h(torch.cat([a2.to_k.weight, a2.to_v.weight], 0), dev)
         p.kv_img = (_h(torch.cat([a2.to_k_ip.weight, a2.to_v_ip.weight], 0), dev) if hasattr(a2, "to_k_ip") else None)
-    else:
-        p.qkv2 = fold_layernorm(torch.cat([a2.to_q.weight, a2.to_k.weight, a2.to_v.weight], 0), None, tb.norm2, dev)
-    p.o2_w, p.o2_b = pack_linear(a2.to_out[0].weight, dev), _f(a2.to_out[0].bias, dev)
     proj = tb.ff.net[0].proj
     p.ff1 = fold_layernorm(proj.weight, proj.bias, tb.norm3, dev, perm=geglu_perm(proj.weight.shape[0]))
     p.ff2_w, p.ff2_b = pack_linear(tb.ff.net[2].weight, dev), _f(tb.ff.net[2].bias, dev)
@@ -151,8 +149,6 @@ class RowStats:
 
     def __init__(self, bld: Builder, rows: int, width: int):
         self.bn = 160 if width in (320, 640) else (256 if width % 256 == 0 else 0)   # producer tile (fixes the slot count)
-        if os.environ.get("TC_ENGINE_ROWSTATS") == "0":                             # A/B: separate tc_row_stats passes
-            self.bn = 0
         self.slots = -(-width // self.bn) if self.bn else 0
         self.bld = bld
         self.buf, self.off = bld.raw(2 * self.slots * rows, torch.float32) if self.bn else (None, None)
@@ -187,63 +183,99 @@ def feed_forward(bld: Builder, x: Act, p: _P, out: Act, stats: Optional[RowStats
     hid.free()
 
 
-def weights_signature(module: nn.Module):
-    """Fingerprint of EVERY parameter and buffer (storage address + in-place version counter).  The module keeps its
-    tensors alive, so an address cannot be recycled while the signature is current; a partial load_state_dict, a LoRA
-    merge or an edit of a late block all bump a version counter and force a re-pack."""
-    return tuple((t.data_ptr(), t._version) for t in list(module.parameters()) + list(module.buffers()))
+def attention_sublayer(bld: Builder, x: Act, a: _P, record, out: Act, s_in: RowStats, s_out: RowStats):
+    """out = x + Wo attention(LN(x) Wproj), with the LayerNorm folded into the projection (statistics `s_in`) and the
+    row statistics of out (`s_out`) written by the output projection; `record(proj, att)` records the attention
+    launch from the projection's output into att."""
+    proj = bld.act(x.N, x.H, x.W, a.proj.w.shape[0])
+    ln_linear(bld, x, a.proj, proj, stats=s_in)
+    att = bld.act(x.N, x.H, x.W, x.C)
+    record(proj, att)
+    proj.free()
+    linear(bld, att, a.o_w, out, bias=a.o_b, res=x, **s_out.producer_kw())
+    att.free()
+
+
+def pack_resblock(dev, norm1, conv1, norm2, conv2, skip=None, time=(), alpha: float = 1.0) -> _P:
+    """ResNet block (UNet ResBlock, VAE ResnetBlock / VideoResBlock): norm1, conv1 (3x3), norm2, conv2 (3x3), the
+    optional 1x1 `skip` conv, and the optional temporal stages `time` [(GroupNorm, (3,1,1) conv)], whose last one
+    blends in the residual with `alpha` (see resblock)."""
+    p = _P(cin=conv1.weight.shape[1], cout=conv1.weight.shape[0], n1=pack_norm(norm1, dev), n2=pack_norm(norm2, dev),
+           c1_w=pack_conv(conv1.weight, dev), c1_b=_f(conv1.bias, dev),
+           c2_w=pack_conv(conv2.weight, dev), c2_b=_f(conv2.bias, dev), skip_w=None, alpha=alpha)
+    if skip is not None:
+        p.skip_w, p.skip_b = pack_linear(skip.weight, dev), _f(skip.bias, dev)
+    p.time = [_P(gn=pack_norm(gn, dev), w=pack_conv(conv.weight, dev), b=_f(conv.bias, dev)) for gn, conv in time]
+    return p
+
+
+def resblock(bld: Builder, p: _P, x: Act, dst: Act, *, B: int = 1, T: int = 1, emb=None) -> None:
+    """GN+SiLU -> 3x3 conv (+ per-sample timestep embedding `emb` [B, cout]) -> GN+SiLU -> 3x3 conv + x (through the
+    1x1 skip when the width changes).  Then, when p.time is set, the temporal stack over the [B][T] frames:
+    [GN over (C/32, T, H, W) -> SiLU -> (3,1,1) conv] per stage, the last one writing dst = s + alpha * conv(...) with s
+    the spatial part's output (UNet TemporalConvBlock: alpha 1, openaimodel3d.py:272-279; VideoResBlock: alpha =
+    sigmoid(mix_factor), autoencoder_dualref.py:892-911)."""
+    N, H, W = x.N, x.H, x.W
+    g1 = bld.act(N, H, W, p.cin)
+    groupnorm(bld, x, g1, p.n1, silu=True)
+    h1 = bld.act(N, H, W, p.cout)
+    gemm(bld, g1, p.c1_w, ops.TAPS_3x3, h1, bias=p.c1_b, bias2=emb, bias2_rows_per=0 if emb is None else T * H * W)
+    g1.free()
+    g2 = bld.act(N, H, W, p.cout)
+    groupnorm(bld, h1, g2, p.n2, silu=True)
+    h1.free()
+    xs = x
+    if p.skip_w is not None:
+        xs = bld.act(N, H, W, p.cout)
+        linear(bld, x, p.skip_w, xs, bias=p.skip_b)
+    s = bld.act(N, H, W, p.cout) if p.time else dst
+    gemm(bld, g2, p.c2_w, ops.TAPS_3x3, s, bias=p.c2_b, res=xs)
+    g2.free()
+    if xs is not x:
+        xs.free()
+    if not p.time:
+        return
+    cur = s
+    for i, tc in enumerate(p.time):
+        g = bld.act(N, H, W, p.cout)
+        groupnorm(bld, cur, g, tc.gn, frames_per_stat=T, silu=True)
+        if cur is not s:
+            cur.free()
+        last = i == len(p.time) - 1
+        nxt = dst if last else bld.act(N, H, W, p.cout)
+        temporal_conv(bld, g, tc.w, nxt, B, bias=tc.b, res=s if last else None, acc_scale=p.alpha if last else 1.0)
+        g.free()
+        cur = nxt
+    s.free()
 
 
 # ------------------------------------------------------------------------------------------------ the UNet engine
-class UNetEngine:
+class UNetEngine(Engine):
     def __init__(self, unet: nn.Module, device=None, arena_bytes: int = 0, use_graph: bool = True,
                  plan_only: bool = False):
-        """plan_only=True builds programs without a GPU (host-logic tests interpret them); it cannot execute."""
+        super().__init__(unet, device, use_graph, plan_only)
         self.lay: UNetLayout = unet.layout
-        p0 = next(unet.parameters())
-        self.dev = torch.device(device) if device is not None else p0.device
-        self.plan_only = plan_only
-        if self.dev.type != "cuda" and not plan_only:
-            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
-        self._sig = weights_signature(unet)
-        self.use_graph = use_graph
         self.arena_bytes = arena_bytes
         self._pack(unet)
-        self._plans: Dict = {}
-
-    def matches(self, unet) -> bool:
-        """True while no parameter of `unet` was replaced, moved or written in place since packing."""
-        p0 = next(unet.parameters())
-        return p0.device == self.dev and self._sig == weights_signature(unet)
 
     # ---------------------------------------------------------------------------------- packing
     def _pack(self, u: nn.Module):
         dev, lay = self.dev, self.lay
-        self.res_blocks: List[_P] = []
         emb_w, emb_b = [], []
         self.emb_cols = 0
 
         def pack_res(m, l: Layer):
-            p = _P(cin=l.cin, cout=l.cout)
-            p.gn1, p.gn2 = pack_norm(m.in_layers[0], dev), pack_norm(m.out_layers[0], dev)
-            p.c1_w, p.c1_b = pack_conv(m.in_layers[2].weight, dev), _f(m.in_layers[2].bias, dev)
-            p.c2_w, p.c2_b = pack_conv(m.out_layers[3].weight, dev), _f(m.out_layers[3].bias, dev)
-            if l.cin != l.cout:
-                p.skip_w, p.skip_b = pack_linear(m.skip_connection.weight, dev), _f(m.skip_connection.bias, dev)
-            else:
-                p.skip_w = None
+            time = ()
+            if hasattr(m, "temopral_conv"):
+                tc = m.temopral_conv
+                time = [(getattr(tc, n)[0], getattr(tc, n)[ci])
+                        for n, ci in (("conv1", 2), ("conv2", 3), ("conv3", 3), ("conv4", 3))]
+            p = pack_resblock(dev, m.in_layers[0], m.in_layers[2], m.out_layers[0], m.out_layers[3],
+                              m.skip_connection if l.cin != l.cout else None, time)
             p.emb_off = self.emb_cols
             self.emb_cols += l.cout
             emb_w.append(m.emb_layers[1].weight.detach())
             emb_b.append(m.emb_layers[1].bias.detach())
-            p.tconv = None
-            if hasattr(m, "temopral_conv"):
-                tc = m.temopral_conv
-                p.tconv = []
-                for name, ci in (("conv1", 2), ("conv2", 3), ("conv3", 3), ("conv4", 3)):
-                    st = getattr(tc, name)
-                    p.tconv.append(_P(gn=pack_norm(st[0], dev), w=pack_conv(st[ci].weight, dev),
-                                      b=_f(st[ci].bias, dev)))
             return p
 
         def pack_tf(m, l: Layer, spatial: bool):
@@ -294,123 +326,44 @@ class UNetEngine:
         self.p_out = _P(gn=pack_norm(u.out[0], dev), w=pack_conv(u.out[2].weight, dev), b=_f(u.out[2].bias, dev))
 
     # ---------------------------------------------------------------------------------- layer builders
-    def _res(self, bld: Builder, p: _P, x: Act, dst: Act, st) -> None:
-        B, T = st["B"], st["T"]
+    def _transformer(self, bld: Builder, p: _P, x: Act, dst: Act, B: int, T: int, kv=None) -> None:
+        """SpatialTransformer (p.spatial: self-attention over the H*W tokens of each frame, cross-attention to the
+        context K/V `kv`) or TemporalTransformer (two self-attentions over the T frames of each pixel)."""
         N, H, W = x.N, x.H, x.W
-        g1 = bld.act(N, H, W, p.cin)
-        groupnorm(bld, x, g1, p.gn1, silu=True)
-        h1 = bld.act(N, H, W, p.cout)
-        emb = st["emb_all"][:, p.emb_off:p.emb_off + p.cout]
-        gemm(bld, g1, p.c1_w, ops.TAPS_3x3, h1, bias=p.c1_b, bias2=emb, bias2_rows_per=T * H * W)
-        g1.free()
-        g2 = bld.act(N, H, W, p.cout)
-        groupnorm(bld, h1, g2, p.gn2, silu=True)
-        h1.free()
-        if p.skip_w is not None:
-            xs = bld.act(N, H, W, p.cout)
-            linear(bld, x, p.skip_w, xs, bias=p.skip_b)
-        else:
-            xs = x
-        if p.tconv is None:
-            gemm(bld, g2, p.c2_w, ops.TAPS_3x3, dst, bias=p.c2_b, res=xs)
-            g2.free()
-            if xs is not x:
-                xs.free()
-            return
-        h2 = bld.act(N, H, W, p.cout)
-        gemm(bld, g2, p.c2_w, ops.TAPS_3x3, h2, bias=p.c2_b, res=xs)
-        g2.free()
-        if xs is not x:
-            xs.free()
-        # temporal conv block: 4 x [GN over (C/32, T, H, W) -> SiLU -> conv (3,1,1)] + identity
-        cur = h2
-        for i, tc in enumerate(p.tconv):
-            g = bld.act(N, H, W, p.cout)
-            groupnorm(bld, cur, g, tc.gn, frames_per_stat=T, silu=True)
-            if cur is not h2:
-                cur.free()
-            last = i == len(p.tconv) - 1
-            nxt = dst if last else bld.act(N, H, W, p.cout)
-            temporal_conv(bld, g, tc.w, nxt, B, bias=tc.b, res=h2 if last else None)
-            g.free()
-            cur = nxt
-        h2.free()
-
-    def _self_attn_spatial(self, bld, x: Act, tb: _P, heads: int, out: Act, s_in: RowStats, s_out: RowStats):
-        qkv = bld.act(x.N, x.H, x.W, 3 * x.C)
-        ln_linear(bld, x, tb.qkv1, qkv, stats=s_in)
-        att = bld.act(x.N, x.H, x.W, x.C)
-        L, C = x.H * x.W, x.C
-        bld.op(ops.attention, qkv.t, [dict(k=qkv.t, v=qkv.t, ldk=3 * C, ldv=3 * C, Lk=L, k_offset=C, v_offset=2 * C)],
-               att.t, q_batches=x.N, Lq=L, heads=heads, scale=64 ** -0.5, ldq=3 * C, ldo=C)
-        qkv.free()
-        linear(bld, att, tb.o1_w, out, bias=tb.o1_b, res=x, **s_out.producer_kw())
-        att.free()
-
-    def _cross_attn(self, bld, x: Act, tb: _P, heads: int, out: Act, kv, st, s_in: RowStats, s_out: RowStats):
-        q = bld.act(x.N, x.H, x.W, x.C)
-        ln_linear(bld, x, tb.q2, q, stats=s_in)
-        att = bld.act(x.N, x.H, x.W, x.C)
-        L, C, T = x.H * x.W, x.C, st["T"]
-        segs = [dict(k=kv["txt"], v=kv["txt"], ldk=2 * C, ldv=2 * C, Lk=kv["n_txt"], kv_div=T, v_offset=C)]
-        if kv["img"] is not None:
-            segs.append(dict(k=kv["img"], v=kv["img"], ldk=2 * C, ldv=2 * C, Lk=kv["n_img"], kv_div=1, v_offset=C))
-        bld.op(ops.attention, q.t, segs, att.t, q_batches=x.N, Lq=L, heads=heads, scale=64 ** -0.5, ldq=C, ldo=C)
-        q.free()
-        linear(bld, att, tb.o2_w, out, bias=tb.o2_b, res=x, **s_out.producer_kw())
-        att.free()
-
-    def _spatial_tf(self, bld: Builder, p: _P, x: Act, dst: Act, st, kv) -> None:
-        N, H, W = x.N, x.H, x.W
+        heads, tb = p.heads, p.tb
         n = bld.act(N, H, W, p.C)
-        groupnorm(bld, x, n, p.norm)
+        groupnorm(bld, x, n, p.norm, frames_per_stat=1 if p.spatial else T)
         # LayerNorm statistics of t0 / t1 / t2 ride the epilogues of the GEMMs that write them
         rows = N * H * W
         s0, s1, s2 = (RowStats(bld, rows, p.inner) for _ in range(3))
         t0 = bld.act(N, H, W, p.inner)
         linear(bld, n, p.in_w, t0, bias=p.in_b, **s0.producer_kw())
         n.free()
+
+        def self_attn(qkv: Act, att: Act):
+            C = att.C
+            if p.spatial:
+                L = att.H * att.W
+                bld.op(ops.attention, qkv.t, [dict(k=qkv.t, v=qkv.t, ldk=3 * C, ldv=3 * C, Lk=L, k_offset=C,
+                                                   v_offset=2 * C)],
+                       att.t, q_batches=att.N, Lq=L, heads=heads, scale=64 ** -0.5, ldq=3 * C, ldo=C)
+            else:
+                bld.op(ops.temporal_attention, qkv.t, qkv.t, qkv.t, att.t, ld=3 * C, ldo=C, B=B, T=T,
+                       P=att.H * att.W, heads=heads, scale=64 ** -0.5, k_offset=C, v_offset=2 * C)
+
+        def cross_attn(q: Act, att: Act):
+            C = att.C
+            segs = [dict(k=kv["txt"], v=kv["txt"], ldk=2 * C, ldv=2 * C, Lk=kv["n_txt"], kv_div=T, v_offset=C)]
+            if kv["img"] is not None:
+                segs.append(dict(k=kv["img"], v=kv["img"], ldk=2 * C, ldv=2 * C, Lk=kv["n_img"], kv_div=1, v_offset=C))
+            bld.op(ops.attention, q.t, segs, att.t, q_batches=att.N, Lq=att.H * att.W, heads=heads, scale=64 ** -0.5,
+                   ldq=C, ldo=C)
+
         t1 = bld.act(N, H, W, p.inner)
-        self._self_attn_spatial(bld, t0, p.tb, p.heads, t1, s0, s1)
+        attention_sublayer(bld, t0, tb.attn1, self_attn, t1, s0, s1)
         t0.free()
         t2 = bld.act(N, H, W, p.inner)
-        self._cross_attn(bld, t1, p.tb, p.heads, t2, kv, st, s1, s2)
-        t1.free()
-        t3 = bld.act(N, H, W, p.inner)
-        feed_forward(bld, t2, p.tb, t3, stats=s2)
-        t2.free()
-        for r in (s0, s1, s2):
-            r.free()
-        linear(bld, t3, p.out_w, dst, bias=p.out_b, res=x)
-        t3.free()
-
-    def _temporal_self_attn(self, bld, x: Act, fqkv: _P, wo, bo, heads: int, out: Act, st, s_in: RowStats,
-                            s_out: RowStats):
-        qkv = bld.act(x.N, x.H, x.W, 3 * x.C)
-        ln_linear(bld, x, fqkv, qkv, stats=s_in)
-        att = bld.act(x.N, x.H, x.W, x.C)
-        C = x.C
-        bld.op(ops.temporal_attention, qkv.t, qkv.t, qkv.t, att.t, ld=3 * C, ldo=C, B=st["B"], T=st["T"], P=x.H * x.W,
-               heads=heads, scale=64 ** -0.5, k_offset=C, v_offset=2 * C)
-        qkv.free()
-        linear(bld, att, wo, out, bias=bo, res=x, **s_out.producer_kw())
-        att.free()
-
-    def _temporal_tf(self, bld: Builder, p: _P, x: Act, dst: Act, st) -> None:
-        N, H, W = x.N, x.H, x.W
-        n = bld.act(N, H, W, p.C)
-        groupnorm(bld, x, n, p.norm, frames_per_stat=st["T"])
-        rows = N * H * W
-        s0, s1, s2 = (RowStats(bld, rows, p.inner) for _ in range(3))
-        t0 = bld.act(N, H, W, p.inner)
-        linear(bld, n, p.in_w, t0, bias=p.in_b, **s0.producer_kw())
-        n.free()
-        tb = p.tb
-        t1 = bld.act(N, H, W, p.inner)
-        self._temporal_self_attn(bld, t0, tb.qkv1, tb.o1_w, tb.o1_b, p.heads, t1, st, s0, s1)
-        t0.free()
-        t2 = bld.act(N, H, W, p.inner)
-        self._temporal_self_attn(bld, t1, tb.qkv2, tb.o2_w, tb.o2_b, p.heads, t2, st, s1, s2)
+        attention_sublayer(bld, t1, tb.attn2, cross_attn if p.spatial else self_attn, t2, s1, s2)
         t1.free()
         t3 = bld.act(N, H, W, p.inner)
         feed_forward(bld, t2, tb, t3, stats=s2)
@@ -421,7 +374,6 @@ class UNetEngine:
         t3.free()
 
     def _down(self, bld: Builder, p: _P, x: Act, dst: Act) -> None:
-        assert x.off == 0 and x.ld == x.C or True
         N, H, W, C = x.N, x.H, x.W, x.C
         src = x
         if x.ld != C or x.off != 0:            # phase split needs a dense tensor
@@ -454,7 +406,6 @@ class UNetEngine:
         arena = Arena(arena_bytes, dev)
         main, ctxp = Program(), Program()
         bld = Builder(arena, main)
-        st = dict(B=B, T=T)
         plan = _P(B=B, T=T, H=H, W=W, arena=arena, main=main, ctx=ctxp)
 
         # static inputs
@@ -466,7 +417,6 @@ class UNetEngine:
         plan.emb = torch.zeros(B, lay.time_dim, dtype=torch.float32, device=dev)
         plan.emb_ws = torch.zeros(B * (lay.model_channels + lay.time_dim), dtype=torch.float32, device=dev)
         plan.emb_all = torch.zeros(B, self.emb_cols, dtype=torch.float16, device=dev)
-        st["emb_all"] = plan.emb_all
         plan.y_out = torch.zeros(B, lay.out_channels, T, H, W, dtype=torch.float16, device=dev)
 
         # --- timestep / fps embeddings -> stacked per-ResBlock embedding vectors
@@ -509,7 +459,7 @@ class UNetEngine:
             if layers[0].kind == "down":
                 h_, w_ = h_ // 2, w_ // 2
             geo.append((h_, w_))
-        cats = []          # per output block: Act of the concat buffer
+        cats = []          # per output block: Act of the concat buffer (never freed: live for the whole program)
         ch = lay.middle_block[-1].cout
         for k, (pref, layers) in enumerate(lay.output_blocks):
             ich = skip_ch[len(skip_ch) - 1 - k]
@@ -547,11 +497,9 @@ class UNetEngine:
                 if p.kind == "conv_in":
                     gemm(bld, x, p.w, ops.TAPS_3x3, dst, bias=p.b)
                 elif p.kind == "res":
-                    self._res(bld, p, x, dst, st)
-                elif p.kind == "st":
-                    self._spatial_tf(bld, p, x, dst, st, kvs[id(p)])
-                elif p.kind == "tt":
-                    self._temporal_tf(bld, p, x, dst, st)
+                    resblock(bld, p, x, dst, B=B, T=T, emb=plan.emb_all[:, p.emb_off:p.emb_off + p.cout])
+                elif p.kind in ("st", "tt"):
+                    self._transformer(bld, p, x, dst, B, T, kvs.get(id(p)))
                 elif p.kind == "down":
                     self._down(bld, p, x, dst)
                 elif p.kind == "up":
@@ -589,8 +537,6 @@ class UNetEngine:
             dst = head_dst(k + 1) if k + 1 < nout else None
             h = run_layers(self.p_output[k], cats[k], dst)
             mark(f"output_blocks.{k}", h)
-        for c in cats:
-            pass           # concat buffers stay allocated for the life of the plan (static program)
         # --- out: GN + SiLU + conv3x3 -> NCTHW fp16
         g = bld.act(N, H, W, h.C)
         groupnorm(bld, h, g, self.p_out.gn, silu=True)
@@ -601,12 +547,6 @@ class UNetEngine:
         return plan
 
     # ---------------------------------------------------------------------------------- execution
-    def plan_for(self, B, T, H, W, n_ctx):
-        key = (B, T, H, W, n_ctx)
-        if key not in self._plans:
-            self._plans[key] = self._build(B, T, H, W, n_ctx)
-        return self._plans[key]
-
     def set_context(self, plan, context: torch.Tensor, executor=None) -> None:
         """Copy the conditioning in and re-run the context K/V program — unconditionally.  Nothing about a caller's
         tensor (address, version counter, shape) identifies its CONTENT once an earlier tensor has been freed: the
@@ -617,7 +557,7 @@ class UNetEngine:
             raise ValueError(f"context {tuple(context.shape)} does not fit the plan ({B}, {plan.n_ctx}, ...)")
         plan.ctx_txt.copy_(context[:, :77].reshape(B * 77, -1))
         plan.ctx_img.copy_(context[:, 77:].reshape(B * T * 16, -1))
-        plan.ctx.run(executor)
+        self._execute(plan.ctx, executor)
 
     def load_inputs(self, plan, x, timesteps, fs) -> None:
         B = plan.B
@@ -633,14 +573,9 @@ class UNetEngine:
     def forward(self, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor, fs=None,
                 executor=None) -> torch.Tensor:
         """`executor` (tests only) interprets the recorded program instead of launching it."""
-        if self.plan_only and executor is None:
-            raise RuntimeError("plan_only engine cannot execute")
         B, _, T, H, W = x.shape
         plan = self.plan_for(B, T, H, W, context.shape[1])
         self.set_context(plan, context, executor)
         self.load_inputs(plan, x, timesteps, fs)
-        if executor is not None:
-            plan.main.run(executor)
-        else:
-            plan.main.replay(self.use_graph)
+        self._execute(plan.main, executor, self.use_graph)
         return plan.y_out

@@ -179,9 +179,7 @@ class UNetModel(nn.Module):
         from . import runtime
         from .engine import UNetEngine
         ex = runtime.TEST_EXECUTOR
-        if self._engine is None or not self._engine.matches(self):
-            self._engine = UNetEngine(self, plan_only=ex is not None)
-        return self._engine.forward(x, timesteps, context, fs, executor=ex).clone()
+        return UNetEngine.cached(self, "_engine", ex).forward(x, timesteps, context, fs, executor=ex).clone()
 
 
 # ----------------------------------------------------------------------------------------------------- VAE parts
@@ -289,9 +287,10 @@ class Resampler(nn.Module):
 
     def forward(self, x):
         """x [B, n_tokens, embedding_dim] (CLIP image tokens) -> [B, num_queries (* video_length), output_dim] fp32."""
+        from . import runtime
         from .cond_engine import ResamplerEngine
-        ex = _clip_engine(self, ResamplerEngine)
-        return self._engine.forward(x, executor=ex).clone()
+        ex = runtime.TEST_EXECUTOR
+        return ResamplerEngine.cached(self, "_engine", ex).forward(x, executor=ex).clone()
 
 
 # ------------------------------------------------------------------------- conditioning: OpenCLIP text / image towers
@@ -418,14 +417,6 @@ def clip_preprocess(x: torch.Tensor, size: int = 224, antialias: bool = True) ->
     return (x - mean) / std
 
 
-def _clip_engine(module, cls):
-    from . import runtime
-    ex = runtime.TEST_EXECUTOR
-    if module._engine is None or not module._engine.matches(module):
-        module._engine = cls(module, plan_only=ex is not None)
-    return ex
-
-
 class FrozenOpenCLIPEmbedder(nn.Module):
     """Drop-in for lvdm.modules.encoders.condition.FrozenOpenCLIPEmbedder (same ctor kwargs; state-dict keys those of
     open_clip's CLIP after `del model.visual`, reference condition.py:184-202).  Downloads nothing: the parameters
@@ -463,9 +454,10 @@ class FrozenOpenCLIPEmbedder(nn.Module):
     def forward(self, text):
         """text: list of strings (or one string), or token ids [B, 77] -> [B, 77, width] fp32."""
         tokens = text if isinstance(text, torch.Tensor) else self.tokenize(text)
+        from . import runtime
         from .cond_engine import ClipTextEngine
-        ex = _clip_engine(self, ClipTextEngine)
-        return self._engine.forward(tokens, executor=ex).clone()
+        ex = runtime.TEST_EXECUTOR
+        return ClipTextEngine.cached(self, "_engine", ex).forward(tokens, executor=ex).clone()
 
     def encode(self, text):
         return self(text)
@@ -511,9 +503,10 @@ class FrozenOpenCLIPImageEmbedderV2(nn.Module):
         return clip_preprocess(x, self.image_size, self.antialias)
 
     def forward(self, image, no_dropout=False):
+        from . import runtime
         from .cond_engine import ClipImageEngine
-        ex = _clip_engine(self, ClipImageEngine)
-        return self._engine.forward(self.preprocess(image), executor=ex).clone()
+        ex = runtime.TEST_EXECUTOR
+        return ClipImageEngine.cached(self, "_engine", ex).forward(self.preprocess(image), executor=ex).clone()
 
     def encode(self, image):
         return self(image)

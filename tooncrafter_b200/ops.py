@@ -36,16 +36,18 @@ TAPS_3x3 = [(dx, dy, 0) for dy in (-1, 0, 1) for dx in (-1, 0, 1)]  # weight ord
 TAPS_T3 = [(0, dt, 0) for dt in (-1, 0, 1)]  # temporal (3,1,1) conv on the [B][T][HW][C] view
 
 
-def taps_3x3_stride2(n_frames: int):
-    """3x3 / stride 2 / pad 1 conv over a phase-split input [4][N][H/2][W/2][C] (tc_phase_split2).
+def taps_3x3_stride2(n_frames: int, pad: int = 1):
+    """3x3 / stride 2 conv over a phase-split input [4][N][H/2][W/2][C] (tc_phase_split2), `pad` zero rows / columns
+    before the image: 1 for the UNet's pad-1 downsample, 0 for the VAE encoder's F.pad(x, (0, 1, 0, 1))
+    (ae_modules.py:104-108).
 
-    input row 2*y + ky - 1  ->  phase row parity (ky-1) & 1, row offset (ky-1) >> 1 (floor).
+    input row 2*y + ky - pad  ->  phase row parity (ky-pad) & 1, row offset (ky-pad) >> 1 (floor).
     """
     taps = []
     for ky in range(3):
         for kx in range(3):
-            py, oy = (ky - 1) & 1, (ky - 1) >> 1
-            px, ox = (kx - 1) & 1, (kx - 1) >> 1
+            py, oy = (ky - pad) & 1, (ky - pad) >> 1
+            px, ox = (kx - pad) & 1, (kx - pad) >> 1
             taps.append((ox, oy, (py * 2 + px) * n_frames))
     return taps
 

@@ -1,4 +1,5 @@
-"""Host runtime shared by the UNet and VAE engines: activation pool, activation views, recorded programs.
+"""Host runtime shared by the network engines: activation pool, activation views, recorded programs, and the engine
+lifecycle (weight fingerprint, plan cache, execution).
 
 Design (H100-first): every network is executed as a STATIC program — a flat list of C-ABI kernel launches over
 pre-allocated channels-last fp16 buffers carved out of one HBM arena — built once per input geometry and then
@@ -160,3 +161,64 @@ class Builder:
 
     def op(self, fn: Callable, *args, **kw) -> None:
         self.prog.add(fn, *args, **kw)
+
+
+def weights_signature(*modules: torch.nn.Module):
+    """Fingerprint of EVERY parameter and buffer (storage address + in-place version counter).  The modules keep their
+    tensors alive, so an address cannot be recycled while the signature is current; a partial load_state_dict, a LoRA
+    merge or an edit of a late block all bump a version counter and force a re-pack."""
+    return tuple((t.data_ptr(), t._version) for m in modules for t in list(m.parameters()) + list(m.buffers()))
+
+
+class Engine:
+    """Lifecycle shared by the network engines: weights packed once from a holder module, one recorded program per
+    input geometry (`plan_for(*key)` -> the subclass's `_build(*key)`, cached in `_plans`), executed by `_execute`.
+
+    plan_only=True builds programs without a GPU (host-logic tests interpret them through an executor); such an engine
+    cannot launch anything."""
+
+    def __init__(self, holder: torch.nn.Module, device=None, use_graph: bool = False, plan_only: bool = False):
+        modules = self._weights(holder)
+        self.dev = torch.device(device) if device is not None else next(modules[0].parameters()).device
+        self.plan_only = plan_only
+        if self.dev.type != "cuda" and not plan_only:
+            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
+        self._sig = weights_signature(*modules)
+        self.use_graph = use_graph
+        self._plans: dict = {}
+
+    @staticmethod
+    def _weights(holder: torch.nn.Module):
+        """The modules whose weights the engine packs from `holder`."""
+        return (holder,)
+
+    def matches(self, holder: torch.nn.Module) -> bool:
+        """True while no weight of `holder` was replaced, moved or written in place since packing."""
+        modules = self._weights(holder)
+        return next(modules[0].parameters()).device == self.dev and self._sig == weights_signature(*modules)
+
+    @classmethod
+    def cached(cls, holder: torch.nn.Module, attr: str, executor: Optional[Callable] = None,
+               module: Optional[torch.nn.Module] = None):
+        """The engine of `module` (default: `holder`) stored in `holder.<attr>`, (re)built when missing or stale;
+        plan-only when an executor will interpret its programs."""
+        module = holder if module is None else module
+        eng = getattr(holder, attr)
+        if eng is None or not eng.matches(module):
+            eng = cls(module, plan_only=executor is not None)
+            setattr(holder, attr, eng)
+        return eng
+
+    def plan_for(self, *key):
+        if key not in self._plans:
+            self._plans[key] = self._build(*key)
+        return self._plans[key]
+
+    def _execute(self, prog: Program, executor: Optional[Callable] = None, use_graph: bool = False) -> None:
+        """Interpret `prog` through `executor` (tests), or launch it: as a captured CUDA graph when `use_graph`."""
+        if executor is not None:
+            prog.run(executor)
+        elif self.plan_only:
+            raise RuntimeError("plan_only engine cannot execute")
+        else:
+            prog.replay(use_graph)

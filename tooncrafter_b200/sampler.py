@@ -228,9 +228,7 @@ class DDIMSampler(object):
         unet = m.model.diffusion_model
         from .engine import UNetEngine
         ex = getattr(self, "_test_executor", None)
-        if unet._engine is None or not unet._engine.matches(unet):
-            unet._engine = UNetEngine(unet, plan_only=ex is not None)
-        eng = unet._engine
+        eng = UNetEngine.cached(unet, "_engine", ex)
         b, c, T, H, W = shape
         group = getattr(self, "latency_group", None)
         if group is not None:
@@ -275,10 +273,7 @@ class DDIMSampler(object):
         for r in range(st.nb // b):                                          # the same latent under every branch
             plan.x_in[r * b:(r + 1) * b, :c].copy_(x)
         plan.t_in.copy_(st.t_table[i].expand(st.nb))
-        if st.ex is None:
-            plan.main.replay(st.eng.use_graph)
-        else:
-            plan.main.run(st.ex)
+        st.eng._execute(plan.main, st.ex, st.eng.use_graph)
         e_img = None
         if st.group is None:
             y = plan.y_out

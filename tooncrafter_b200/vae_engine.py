@@ -18,74 +18,77 @@ reference-frame K/V projections are computed once per clip, and the mid-block so
 """
 from __future__ import annotations
 
-import math
-from typing import Dict, List
+from typing import List
 
 import torch
 import torch.nn as nn
 
 from . import ops
-from .engine import (_P, _f, _h, gemm, groupnorm, linear, pack_conv, pack_linear, pack_norm, temporal_conv,
-                     weights_signature)
+from .engine import (_P, _f, _h, gemm, groupnorm, linear, pack_conv, pack_linear, pack_norm, pack_resblock, resblock,
+                     temporal_conv)
 from .layout import DecoderLayout
-from .runtime import Act, Arena, Builder, Program
+from .runtime import Act, Arena, Builder, Engine, Program
 
 
-class DecoderEngine:
+def pack_vae_resnet(m, dev) -> _P:
+    """ResnetBlock, or VideoResBlock when it has a time_stack (alpha = sigmoid(mix_factor))."""
+    skip = getattr(m, "nin_shortcut", None)
+    ts = getattr(m, "time_stack", None)
+    if ts is None:
+        return pack_resblock(dev, m.norm1, m.conv1, m.norm2, m.conv2, skip)
+    mf = m.mix_factor.detach().float()
+    alpha = 0.5 if mf.is_meta else float(torch.sigmoid(mf).item())    # meta: planning-only engines (host tests)
+    return pack_resblock(dev, m.norm1, m.conv1, m.norm2, m.conv2, skip,
+                         ((ts.in_layers[0], ts.in_layers[2]), (ts.out_layers[0], ts.out_layers[3])), alpha)
+
+
+def pack_mid_attention(a, C: int, dev) -> _P:
+    return _P(C=C, norm=pack_norm(a.norm, dev),
+              qkv_w=_h(torch.cat([a.q.weight.reshape(C, C), a.k.weight.reshape(C, C), a.v.weight.reshape(C, C)], 0), dev),
+              qkv_b=_f(torch.cat([a.q.bias, a.k.bias, a.v.bias], 0), dev),
+              o_w=pack_linear(a.proj_out.weight, dev), o_b=_f(a.proj_out.bias, dev))
+
+
+def mid_attention(bld: Builder, p: _P, x: Act, dst: Act) -> None:
+    """AttnBlock (autoencoder_dualref.py:172-206, ae_modules.py:28-75): GroupNorm -> fused q/k/v 1x1 convs -> one fused
+    single-head attention kernel per call (head dim = C, scores never leave the SM) -> proj_out + residual."""
+    N, H, W, C = x.N, x.H, x.W, p.C
+    if C % 64 or C > 512 or (C > 256 and C % 128):
+        raise NotImplementedError(f"mid-block attention: {C} channels (tc_attention_wide takes multiples of 64 up to 512, "
+                                  f"of 128 above 256)")
+    n = bld.act(N, H, W, C)
+    groupnorm(bld, x, n, p.norm)
+    qkv = bld.act(N, H, W, 3 * C)
+    linear(bld, n, p.qkv_w, qkv, bias=p.qkv_b)
+    n.free()
+    att = bld.act(N, H, W, C)
+    bld.op(ops.attention_wide, qkv.t, att.t, batches=N, L=H * W, D=C, scale=C ** -0.5, ld=3 * C, ldo=C,
+           q_offset=0, k_offset=C, v_offset=2 * C)
+    qkv.free()
+    linear(bld, att, p.o_w, dst, bias=p.o_b, res=x)
+    att.free()
+
+
+class DecoderEngine(Engine):
     def __init__(self, decoder: nn.Module, device=None, arena_bytes: int = 0, use_graph: bool = True,
                  plan_only: bool = False):
+        super().__init__(decoder, device, use_graph, plan_only)
         self.lay: DecoderLayout = decoder.layout
-        p0 = next(decoder.parameters())
-        self.dev = torch.device(device) if device is not None else p0.device
-        self.plan_only = plan_only
-        if self.dev.type != "cuda" and not plan_only:
-            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
-        self._sig = weights_signature(decoder)
-        self.use_graph = use_graph
         self.arena_bytes = arena_bytes
         self._pack(decoder)
-        self._plans: Dict = {}
-
-    def matches(self, decoder) -> bool:
-        p0 = next(decoder.parameters())
-        return p0.device == self.dev and self._sig == weights_signature(decoder)
 
     # ---------------------------------------------------------------------------------- packing
     def _pack(self, d: nn.Module):
         dev, lay = self.dev, self.lay
-
-        def res(m):
-            cin, cout = m.conv1.weight.shape[1], m.conv1.weight.shape[0]
-            p = _P(cin=cin, cout=cout)
-            p.n1, p.n2 = pack_norm(m.norm1, dev), pack_norm(m.norm2, dev)
-            p.c1_w, p.c1_b = pack_conv(m.conv1.weight, dev), _f(m.conv1.bias, dev)
-            p.c2_w, p.c2_b = pack_conv(m.conv2.weight, dev), _f(m.conv2.bias, dev)
-            if hasattr(m, "nin_shortcut"):
-                p.nin_w, p.nin_b = pack_linear(m.nin_shortcut.weight, dev), _f(m.nin_shortcut.bias, dev)
-            else:
-                p.nin_w = None
-            ts = m.time_stack
-            p.tn1, p.tn2 = pack_norm(ts.in_layers[0], dev), pack_norm(ts.out_layers[0], dev)
-            p.t1_w, p.t1_b = pack_conv(ts.in_layers[2].weight, dev), _f(ts.in_layers[2].bias, dev)
-            p.t2_w, p.t2_b = pack_conv(ts.out_layers[3].weight, dev), _f(ts.out_layers[3].bias, dev)
-            mf = m.mix_factor.detach().float()
-            p.alpha = 0.5 if mf.is_meta else float(torch.sigmoid(mf).item())    # meta: planning-only engines (host tests)
-            return p
-
         self.cpad_in = (lay.z_channels + 63) // 64 * 64
         self.p_conv_in = _P(w=pack_conv(d.conv_in.weight, dev, self.cpad_in), b=_f(d.conv_in.bias, dev))
-        self.p_mid1, self.p_mid2 = res(d.mid.block_1), res(d.mid.block_2)
-        a = d.mid.attn_1
-        C = lay.block_in
-        self.p_attn = _P(C=C, norm=pack_norm(a.norm, dev),
-                         qkv_w=_h(torch.cat([a.q.weight.reshape(C, C), a.k.weight.reshape(C, C), a.v.weight.reshape(C, C)], 0), dev),
-                         qkv_b=_f(torch.cat([a.q.bias, a.k.bias, a.v.bias], 0), dev),
-                         o_w=pack_linear(a.proj_out.weight, dev), o_b=_f(a.proj_out.bias, dev))
+        self.p_mid1, self.p_mid2 = pack_vae_resnet(d.mid.block_1, dev), pack_vae_resnet(d.mid.block_2, dev)
+        self.p_attn = pack_mid_attention(d.mid.attn_1, lay.block_in, dev)
         self.p_levels: List[_P] = []
         for i, lv in enumerate(lay.levels):
             up = d.up[i]
             p = _P(channels=lv["channels"], refine=lv["refine"], upsample=lv["upsample"])
-            p.blocks = [res(up.block[j]) for j in range(len(lv["blocks"]))]
+            p.blocks = [pack_vae_resnet(up.block[j], dev) for j in range(len(lv["blocks"]))]
             r = d.attn_refinement[i]
             if lv["refine"] == "fusion":
                 heads = r.to_q.weight.shape[0] // 64
@@ -105,58 +108,6 @@ class DecoderEngine:
                           tmix_b=_f(d.conv_out.time_mix_conv.bias, dev))
 
     # ---------------------------------------------------------------------------------- builders
-    def _video_res(self, bld: Builder, p: _P, x: Act, dst: Act, T: int) -> None:
-        N, H, W = x.N, x.H, x.W
-        g1 = bld.act(N, H, W, p.cin)
-        groupnorm(bld, x, g1, p.n1, silu=True)
-        h1 = bld.act(N, H, W, p.cout)
-        gemm(bld, g1, p.c1_w, ops.TAPS_3x3, h1, bias=p.c1_b)
-        g1.free()
-        g2 = bld.act(N, H, W, p.cout)
-        groupnorm(bld, h1, g2, p.n2, silu=True)
-        h1.free()
-        if p.nin_w is not None:
-            xs = bld.act(N, H, W, p.cout)
-            linear(bld, x, p.nin_w, xs, bias=p.nin_b)
-        else:
-            xs = x
-        s = bld.act(N, H, W, p.cout)
-        gemm(bld, g2, p.c2_w, ops.TAPS_3x3, s, bias=p.c2_b, res=xs)
-        g2.free()
-        if xs is not x:
-            xs.free()
-        # time stack: GN (stats over all T frames) -> SiLU -> conv (3,1,1), twice; alpha blend in the epilogue
-        g3 = bld.act(N, H, W, p.cout)
-        groupnorm(bld, s, g3, p.tn1, frames_per_stat=T, silu=True)
-        h3 = bld.act(N, H, W, p.cout)
-        temporal_conv(bld, g3, p.t1_w, h3, 1, bias=p.t1_b)
-        g3.free()
-        g4 = bld.act(N, H, W, p.cout)
-        groupnorm(bld, h3, g4, p.tn2, frames_per_stat=T, silu=True)
-        h3.free()
-        temporal_conv(bld, g4, p.t2_w, dst, 1, bias=p.t2_b, res=s, acc_scale=p.alpha)
-        g4.free()
-        s.free()
-
-    def _mid_attention(self, bld: Builder, p: _P, x: Act, dst: Act) -> None:   # also used by EncoderEngine (self unused)
-        """AttnBlock (autoencoder_dualref.py:172-206): GroupNorm -> fused q/k/v 1x1 convs -> one fused single-head attention
-        kernel per call (head dim = C, scores never leave the SM) -> proj_out + residual."""
-        N, H, W, C = x.N, x.H, x.W, p.C
-        if C % 64 or C > 512 or (C > 256 and C % 128):
-            raise NotImplementedError(f"mid-block attention: {C} channels (tc_attention_wide takes multiples of 64 up to 512, "
-                                      f"of 128 above 256)")
-        n = bld.act(N, H, W, C)
-        groupnorm(bld, x, n, p.norm)
-        qkv = bld.act(N, H, W, 3 * C)
-        linear(bld, n, p.qkv_w, qkv, bias=p.qkv_b)
-        n.free()
-        att = bld.act(N, H, W, C)
-        bld.op(ops.attention_wide, qkv.t, att.t, batches=N, L=H * W, D=C, scale=C ** -0.5, ld=3 * C, ldo=C,
-               q_offset=0, k_offset=C, v_offset=2 * C)
-        qkv.free()
-        linear(bld, att, p.o_w, dst, bias=p.o_b, res=x)
-        att.free()
-
     def _fusion(self, bld: Builder, p: _P, x: Act, dst: Act, kv: torch.Tensor, n_kv: int) -> None:
         N, H, W, C = x.N, x.H, x.W, x.C
         n = bld.act(N, H, W, C)
@@ -220,17 +171,17 @@ class DecoderEngine:
         plan.marks = []
 
         nxt = bld.act(T, h, w, lay.block_in)
-        self._video_res(bld, self.p_mid1, cur, nxt, T); cur.free(); cur = nxt
+        resblock(bld, self.p_mid1, cur, nxt, T=T); cur.free(); cur = nxt
         nxt = bld.act(T, h, w, lay.block_in)
-        self._mid_attention(bld, self.p_attn, cur, nxt); cur.free(); cur = nxt
+        mid_attention(bld, self.p_attn, cur, nxt); cur.free(); cur = nxt
         nxt = bld.act(T, h, w, lay.block_in)
-        self._video_res(bld, self.p_mid2, cur, nxt, T); cur.free(); cur = nxt
+        resblock(bld, self.p_mid2, cur, nxt, T=T); cur.free(); cur = nxt
         plan.marks.append((len(main), "mid", cur))
         for i in reversed(range(nlev)):
             p = self.p_levels[i]
             for rb in p.blocks:
                 nxt = bld.act(T, cur.H, cur.W, rb.cout)
-                self._video_res(bld, rb, cur, nxt, T); cur.free(); cur = nxt
+                resblock(bld, rb, cur, nxt, T=T); cur.free(); cur = nxt
             if p.refine == "fusion":
                 nxt = bld.act(T, cur.H, cur.W, cur.C)
                 kv, n_kv = plan.kv[i]
@@ -263,12 +214,6 @@ class DecoderEngine:
         main.add(ops.cl_to_ncthw, fin.t, plan.y_out, B=T, C_=lay.out_ch, T=1, H=Hf, W=Wf, ldx=16)
         return plan
 
-    def plan_for(self, T, h, w):
-        key = (T, h, w)
-        if key not in self._plans:
-            self._plans[key] = self._build(T, h, w)
-        return self._plans[key]
-
     def set_ref_context(self, plan, ref_context, executor=None) -> None:
         """Copy the reference-frame maps in and re-run the packing / fusion-K/V program on EVERY decode: tensor
         addresses recycle between clips (the maps are per-clip temporaries), so no pointer-derived key may skip it.
@@ -280,38 +225,23 @@ class DecoderEngine:
                 raise ValueError(f"ref_context map {tuple(src.shape)} != expected {tuple(dst.shape)} "
                                  "(one clip per decode call: batch must be 1)")
             dst.copy_(src)
-        plan.ctx.run(executor)
+        self._execute(plan.ctx, executor)
 
     @torch.no_grad()
     def decode(self, z: torch.Tensor, ref_context, executor=None) -> torch.Tensor:
         """z [T, z_channels, h, w] (already divided by scale_factor), ref_context: 5 maps [1, C, 2, H_l, W_l]
         -> [T, 3, 8h, 8w] fp16."""
-        if self.plan_only and executor is None:
-            raise RuntimeError("plan_only engine cannot execute")
         if ref_context is None:
             raise NotImplementedError("VideoDecoder without ref_context is outside the supported hot path")
         T, _, h, w = z.shape
         plan = self.plan_for(T, h, w)
         self.set_ref_context(plan, ref_context, executor)
         plan.z_in.copy_(z.reshape(plan.z_in.shape))
-        if executor is not None:
-            plan.main.run(executor)
-        else:
-            plan.main.replay(self.use_graph)
+        self._execute(plan.main, executor, self.use_graph)
         return plan.y_out.reshape(T, self.lay.out_ch, plan.y_out.shape[-2], plan.y_out.shape[-1])
 
 
-def taps_3x3_stride2_pad_br(n_frames: int):
-    """3x3 / stride 2 conv after F.pad(x, (0, 1, 0, 1)) (ae_modules.py:104-108) over a phase-split input:
-    input row 2*y + ky  ->  phase row parity ky & 1, row offset ky >> 1."""
-    taps = []
-    for ky in range(3):
-        for kx in range(3):
-            taps.append((kx >> 1, ky >> 1, ((ky & 1) * 2 + (kx & 1)) * n_frames))
-    return taps
-
-
-class EncoderEngine:
+class EncoderEngine(Engine):
     """AutoencoderKL.encode(x, return_hidden_states=True): Encoder + quant_conv.
 
     Reference: lvdm/modules/networks/ae_modules.py:432-475 (Encoder.forward), :153-213 (ResnetBlock), :28-75
@@ -319,77 +249,34 @@ class EncoderEngine:
 
     def __init__(self, ae: nn.Module, device=None, arena_bytes: int = 0, use_graph: bool = False,
                  plan_only: bool = False):
-        enc = ae.encoder
-        self.lay = enc.layout
-        p0 = next(enc.parameters())
-        self.dev = torch.device(device) if device is not None else p0.device
-        self.plan_only = plan_only
-        if self.dev.type != "cuda" and not plan_only:
-            raise RuntimeError("tooncrafter_b200 runs on CUDA only (no CPU fallback); move the model to a GPU")
-        self._sig = weights_signature(ae.encoder) + weights_signature(ae.quant_conv)
-        self.use_graph = use_graph
+        super().__init__(ae, device, use_graph, plan_only)
+        self.lay = ae.encoder.layout
         self.arena_bytes = arena_bytes
         self._pack(ae)
-        self._plans: Dict = {}
 
-    def matches(self, ae) -> bool:
-        p0 = next(ae.encoder.parameters())
-        return p0.device == self.dev and self._sig == weights_signature(ae.encoder) + weights_signature(ae.quant_conv)
+    @staticmethod
+    def _weights(ae):
+        return (ae.encoder, ae.quant_conv)
 
     def _pack(self, ae):
         dev, lay, e = self.dev, self.lay, ae.encoder
-
-        def res(m):
-            cin, cout = m.conv1.weight.shape[1], m.conv1.weight.shape[0]
-            p = _P(cin=cin, cout=cout, n1=pack_norm(m.norm1, dev), n2=pack_norm(m.norm2, dev),
-                   c1_w=pack_conv(m.conv1.weight, dev), c1_b=_f(m.conv1.bias, dev),
-                   c2_w=pack_conv(m.conv2.weight, dev), c2_b=_f(m.conv2.bias, dev), nin_w=None)
-            if hasattr(m, "nin_shortcut"):
-                p.nin_w, p.nin_b = pack_linear(m.nin_shortcut.weight, dev), _f(m.nin_shortcut.bias, dev)
-            return p
-
         self.cpad_in = (lay.in_channels + 63) // 64 * 64
         self.p_conv_in = _P(w=pack_conv(e.conv_in.weight, dev, self.cpad_in), b=_f(e.conv_in.bias, dev))
         self.p_levels = []
         for i, lv in enumerate(lay.levels):
             d = e.down[i]
-            p = _P(blocks=[res(d.block[j]) for j in range(len(lv["blocks"]))], down=lv["downsample"],
+            p = _P(blocks=[pack_vae_resnet(d.block[j], dev) for j in range(len(lv["blocks"]))], down=lv["downsample"],
                    channels=lv["channels"])
             if lv["downsample"]:
                 p.down_w, p.down_b = pack_conv(d.downsample.conv.weight, dev), _f(d.downsample.conv.bias, dev)
             self.p_levels.append(p)
-        self.p_mid1, self.p_mid2 = res(e.mid.block_1), res(e.mid.block_2)
-        a, C = e.mid.attn_1, lay.block_in
-        self.p_attn = _P(C=C, norm=pack_norm(a.norm, dev),
-                         qkv_w=_h(torch.cat([a.q.weight.reshape(C, C), a.k.weight.reshape(C, C), a.v.weight.reshape(C, C)], 0), dev),
-                         qkv_b=_f(torch.cat([a.q.bias, a.k.bias, a.v.bias], 0), dev),
-                         o_w=pack_linear(a.proj_out.weight, dev), o_b=_f(a.proj_out.bias, dev))
+        self.p_mid1, self.p_mid2 = pack_vae_resnet(e.mid.block_1, dev), pack_vae_resnet(e.mid.block_2, dev)
+        self.p_attn = pack_mid_attention(e.mid.attn_1, lay.block_in, dev)
         self.zc2 = e.conv_out.weight.shape[0]
         self.p_out = _P(norm=pack_norm(e.norm_out, dev), w=pack_conv(e.conv_out.weight, dev), b=_f(e.conv_out.bias, dev),
                         q_w=_h(torch.nn.functional.pad(ae.quant_conv.weight.detach().reshape(ae.quant_conv.weight.shape[0], -1),
                                                        (0, 64 - self.zc2)), dev),
                         q_b=_f(ae.quant_conv.bias, dev), q_out=ae.quant_conv.weight.shape[0])
-
-    @staticmethod
-    def _resnet2d(bld: Builder, p: _P, x: Act, dst: Act) -> None:
-        N, H, W = x.N, x.H, x.W
-        g1 = bld.act(N, H, W, p.cin)
-        groupnorm(bld, x, g1, p.n1, silu=True)
-        h1 = bld.act(N, H, W, p.cout)
-        gemm(bld, g1, p.c1_w, ops.TAPS_3x3, h1, bias=p.c1_b)
-        g1.free()
-        g2 = bld.act(N, H, W, p.cout)
-        groupnorm(bld, h1, g2, p.n2, silu=True)
-        h1.free()
-        if p.nin_w is not None:
-            xs = bld.act(N, H, W, p.cout)
-            linear(bld, x, p.nin_w, xs, bias=p.nin_b)
-        else:
-            xs = x
-        gemm(bld, g2, p.c2_w, ops.TAPS_3x3, dst, bias=p.c2_b, res=xs)
-        g2.free()
-        if xs is not x:
-            xs.free()
 
     def _build(self, N: int, H: int, W: int):
         lay, dev = self.lay, self.dev
@@ -417,7 +304,7 @@ class EncoderEngine:
         for p in self.p_levels:
             for rb in p.blocks:
                 nxt = bld.act(N, cur.H, cur.W, rb.cout)
-                self._resnet2d(bld, rb, cur, nxt)
+                resblock(bld, rb, cur, nxt)
                 cur.free()
                 cur = nxt
             plan.hidden.append(export(cur))
@@ -425,17 +312,17 @@ class EncoderEngine:
                 ph = bld.act(4 * N, cur.H // 2, cur.W // 2, cur.C)
                 bld.op(ops.phase_split2, cur.t, ph.t, N=N, H=cur.H, W=cur.W, C_=cur.C)
                 nxt = bld.act(N, cur.H // 2, cur.W // 2, cur.C)
-                gemm(bld, ph, p.down_w, taps_3x3_stride2_pad_br(N), nxt, bias=p.down_b)
+                gemm(bld, ph, p.down_w, ops.taps_3x3_stride2(N, pad=0), nxt, bias=p.down_b)
                 ph.free()
                 cur.free()
                 cur = nxt
         plan.hidden.append(first_out)
         nxt = bld.act(N, cur.H, cur.W, cur.C)
-        self._resnet2d(bld, self.p_mid1, cur, nxt); cur.free(); cur = nxt
+        resblock(bld, self.p_mid1, cur, nxt); cur.free(); cur = nxt
         nxt = bld.act(N, cur.H, cur.W, cur.C)
-        DecoderEngine._mid_attention(None, bld, self.p_attn, cur, nxt); cur.free(); cur = nxt
+        mid_attention(bld, self.p_attn, cur, nxt); cur.free(); cur = nxt
         nxt = bld.act(N, cur.H, cur.W, cur.C)
-        self._resnet2d(bld, self.p_mid2, cur, nxt); cur.free(); cur = nxt
+        resblock(bld, self.p_mid2, cur, nxt); cur.free(); cur = nxt
         g = bld.act(N, cur.H, cur.W, cur.C)
         groupnorm(bld, cur, g, self.p_out.norm, silu=True)
         cur.free()
@@ -452,17 +339,9 @@ class EncoderEngine:
     @torch.no_grad()
     def encode(self, x: torch.Tensor, executor=None):
         """x [N, 3, H, W] in [-1, 1] -> (moments [N, 2*embed, H/8, W/8] fp32, [5 hidden maps [N, C, H_l, W_l] fp16])."""
-        if self.plan_only and executor is None:
-            raise RuntimeError("plan_only engine cannot execute")
         N, _, H, W = x.shape
-        key = (N, H, W)
-        if key not in self._plans:
-            self._plans[key] = self._build(N, H, W)
-        plan = self._plans[key]
+        plan = self.plan_for(N, H, W)
         plan.x_in.copy_(x.reshape(plan.x_in.shape))
-        if executor is not None:
-            plan.main.run(executor)
-        else:
-            plan.main.replay(self.use_graph)
+        self._execute(plan.main, executor, self.use_graph)
         sq = lambda t: t.reshape(t.shape[0], t.shape[1], t.shape[3], t.shape[4]).clone()
         return sq(plan.moments), [sq(h) for h in plan.hidden]
