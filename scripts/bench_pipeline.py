@@ -7,7 +7,15 @@ For K = 2 and K = 5 keyframes it times, alternating in one process, two ways to 
 Each arm is warmed up once at DDIM-2 (plans, graphs), then timed `--reps` times with the device synchronised.
 Prints the GPU name and power limit (nvidia-smi) and one JSON line.
 
-    python scripts/bench_pipeline.py [--reps 2] [--ddim-steps 50]
+    python scripts/bench_pipeline.py [--reps 2] [--ddim-steps 50] [--first-stage plain|dualref] [--size H W]
+
+--animate measures the single-image path instead, at --size with --first-stage: seconds per video and frames/s of
+ToonCrafterPipeline.animate and of a K = 2 interpolate() (warm-up, then `--reps` timed runs each, alternating), the
+peak device memory of each, the peak of a default K = 5 interpolate() call (segments_per_batch 4, DDIM-2: memory does
+not depend on the step count), and the first-stage decode of 16 latents, plain against dual-reference decoder (CUDA
+events, 10 replays after a warm-up):
+
+    python scripts/bench_pipeline.py --animate --first-stage plain --size 576 1024
 """
 from __future__ import annotations
 
@@ -25,10 +33,12 @@ sys.path.insert(0, str(ROOT))
 sys.path.insert(0, str(ROOT / "tests"))
 
 
-def full_pipeline_config():
-    """configs/inference_512_v1.0.yaml with the OpenCLIP towers and the Resampler of this repository."""
+def full_pipeline_config(size=(320, 512)):
+    """configs/inference_512_v1.0.yaml with the OpenCLIP towers and the Resampler of this repository (image_size:
+    the latent of `size`, as configs/training_1024_v1.0 sets [72, 128] for 576 x 1024)."""
     from tiny_config import FULL_DDCONFIG, FULL_UNET, model_config
     cfg = model_config(FULL_UNET, FULL_DDCONFIG)
+    cfg["params"]["image_size"] = [size[0] // 8, size[1] // 8]
     p = cfg["params"]
     p["cond_stage_config"] = {"target": "tooncrafter_b200.modules.FrozenOpenCLIPEmbedder",
                               "params": {"freeze": True, "layer": "penultimate"}}
@@ -50,10 +60,95 @@ def gpu_info():
         return dict(name=torch.cuda.get_device_name(), power_limit=f"unavailable ({type(e).__name__})")
 
 
+def _timed(fn):
+    torch.cuda.synchronize()
+    torch.cuda.reset_peak_memory_stats()
+    t = time.perf_counter()
+    fn()
+    torch.cuda.synchronize()
+    return time.perf_counter() - t, torch.cuda.max_memory_allocated()
+
+
+def decode_ms(size, reps=10):
+    """ms per decode of 16 latents at `size`, plain AutoencoderKL vs AutoencoderKL_Dualref (full width, synthetic
+    weights, the dual-reference decoder with its reference-frame maps), each engine's program replayed as a graph."""
+    from tiny_config import FULL_DDCONFIG
+    from tooncrafter_b200 import diffusion, synthetic
+    h, w = size[0] // 8, size[1] // 8
+    z = torch.randn(16, 4, h, w, generator=torch.Generator().manual_seed(1)).cuda() * 3.0
+    out = {}
+    for name, cls in (("plain", diffusion.AutoencoderKL), ("dualref", diffusion.AutoencoderKL_Dualref)):
+        with torch.device("meta"):
+            sk = cls(ddconfig=FULL_DDCONFIG, embed_dim=4)
+        ae = sk.to_empty(device="cuda")
+        with torch.no_grad():
+            for k, p in ae.named_parameters():
+                p.copy_(synthetic.synthetic_tensor("first_stage_model." + k, tuple(p.shape), 0).cuda())
+        eng = ae.decoder_engine()
+        if name == "plain":
+            run = lambda: eng.decode(z)                                                      # noqa: E731
+        else:
+            ref = [r.cuda() for r in synthetic.synthetic_ref_context(FULL_DDCONFIG["ch"], FULL_DDCONFIG["ch_mult"],
+                                                                     size[0], size[1])]
+            run = lambda: eng.decode(z, ref)                                                 # noqa: E731
+        run()
+        torch.cuda.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(reps):
+            run()
+        e1.record()
+        torch.cuda.synchronize()
+        out[name] = e0.elapsed_time(e1) / reps
+        del eng, ae
+        torch.cuda.empty_cache()
+    return out
+
+
+def bench_animate(args, model, info, build_s, decode16):
+    """animate and K = 2 interpolate at args.size (see the module docstring)."""
+    from tooncrafter_b200.pipeline import ToonCrafterPipeline
+    size = tuple(args.size)
+    pipe = ToonCrafterPipeline(model)
+    g = torch.Generator().manual_seed(0)
+    kf = (torch.rand(5, size[0], size[1], 3, generator=g) * 255).to(torch.uint8)
+    arms = dict(animate=(lambda st: pipe.animate(kf[0], steps=st, seed=123, size=size), 16),
+                interpolate_k2=(lambda st: pipe.interpolate(kf[:2], steps=st, seed=123, size=size), 16))
+    for fn, _ in arms.values():
+        fn(2)
+    times = {name: [] for name in arms}
+    peaks = {name: 0 for name in arms}
+    for _ in range(args.reps):
+        for name, (fn, _) in arms.items():
+            t, peak = _timed(lambda: fn(args.ddim_steps))
+            times[name].append(t)
+            peaks[name] = max(peaks[name], peak)
+    row = {}
+    for name, (_, F) in arms.items():
+        best = min(times[name])
+        row[name] = dict(frames=F, sec_per_video=best, frames_per_s=F / best, all_s=[round(x, 3) for x in times[name]],
+                         peak_mem_gib=peaks[name] / 2 ** 30)
+    _, peak5 = _timed(lambda: pipe.interpolate(kf, steps=2, seed=123, size=size))
+    row["interpolate_k5_default_peak_mem_gib"] = peak5 / 2 ** 30
+    row["decode16_ms"] = decode16
+    out = dict(metric="single-image animate and K=2 interpolation: seconds per video (%dx%d, DDIM-%d, CFG 7.5, eta 1, "
+               "synthetic weights, %s first stage)" % (size[0], size[1], args.ddim_steps, args.first_stage),
+               gpu=info, reps=args.reps, model_build_s=build_s, first_stage=args.first_stage, size=list(size), **row,
+               note="sec_per_video = best of the timed reps, host clock around work ending in a device synchronise; "
+                    "peak_mem = torch.cuda.max_memory_allocated over the call (model and cached plans included); "
+                    "decode16_ms = CUDA events over 10 graph replays of one 16-latent decode")
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=2)
     ap.add_argument("--ddim-steps", type=int, default=50)
+    ap.add_argument("--first-stage", choices=("dualref", "plain"), default="dualref",
+                    help="AutoencoderKL_Dualref (ToonCrafter) or the plain AutoencoderKL (DynamiCrafter / training configs)")
+    ap.add_argument("--size", type=int, nargs=2, default=(320, 512), metavar=("H", "W"))
+    ap.add_argument("--animate", action="store_true", help="measure animate and K = 2 interpolation (docstring)")
     args = ap.parse_args()
     from tooncrafter_b200 import synthetic
     from tooncrafter_b200.pipeline import ToonCrafterPipeline
@@ -63,22 +158,27 @@ def main():
     info = gpu_info()
     print(f"GPU: {info['name']}, power limit {info['power_limit']}", flush=True)
     torch.backends.cuda.matmul.allow_tf32 = False
+    size = tuple(args.size)
+    decode16 = decode_ms(size) if args.animate else None       # before the model: the two decoders' plans alone
+    torch.cuda.empty_cache()
     t0 = time.perf_counter()
-    model = synthetic.synthetic_model(full_pipeline_config(), dev)
+    model = synthetic.synthetic_model(full_pipeline_config(size), dev, first_stage=args.first_stage)
     model.perframe_ae = True
     build_s = time.perf_counter() - t0
+    if args.animate:
+        return bench_animate(args, model, info, build_s, decode16)
     pipe = ToonCrafterPipeline(model)
     g = torch.Generator().manual_seed(0)
     results = []
     for K in (2, 5):
-        kf = (torch.rand(K, 320, 512, 3, generator=g) * 255).to(torch.uint8)
+        kf = (torch.rand(K, size[0], size[1], 3, generator=g) * 255).to(torch.uint8)
         S = K - 1
 
         def batched(steps):
-            return pipe.interpolate(kf, steps=steps, seed=123)
+            return pipe.interpolate(kf, steps=steps, seed=123, size=size)
 
         def pairs(steps):
-            return [pipe.interpolate(kf[k:k + 2], steps=steps, seed=123 + k) for k in range(S)]
+            return [pipe.interpolate(kf[k:k + 2], steps=steps, seed=123 + k, size=size) for k in range(S)]
 
         arms = dict(batched=batched, pairs=pairs)
         for fn in arms.values():
@@ -100,8 +200,8 @@ def main():
         row["batched_over_pairs_time"] = row["batched"]["sec_per_video"] / row["pairs"]["sec_per_video"]
         results.append(row)
         print(json.dumps(row), flush=True)
-    out = dict(metric="keyframe interpolation: seconds per video (320x512, DDIM-%d, CFG 7.5, eta 1, synthetic weights)"
-               % args.ddim_steps, gpu=info, reps=args.reps, model_build_s=build_s, configs=results,
+    out = dict(metric="keyframe interpolation: seconds per video (%dx%d, DDIM-%d, CFG 7.5, eta 1, synthetic weights, "
+               "%s first stage)" % (size[0], size[1], args.ddim_steps, args.first_stage), gpu=info, reps=args.reps, model_build_s=build_s, configs=results,
                note="sec_per_video = best of the timed reps, host clock around work ending in a device synchronise; "
                     "frames counts the joined video (15 * segments + 1)")
     print(json.dumps(out), flush=True)

@@ -116,8 +116,7 @@ class AutoencoderKL(nn.Module):
             self.load_state_dict(sd.get("state_dict", sd), strict=False)
 
     def _make_decoder(self, dd):
-        raise NotImplementedError("plain AutoencoderKL decoder is outside the supported hot path; "
-                                  "use AutoencoderKL_Dualref")
+        return modules.Decoder(**dd)
 
     @property
     def device(self):
@@ -130,6 +129,27 @@ class AutoencoderKL(nn.Module):
         moments, hidden = EncoderEngine.cached(self, "_enc_engine", ex).encode(x, executor=ex)
         post = DiagonalGaussianDistribution(moments)
         return (post, hidden) if return_hidden_states else post
+
+    def decode(self, z, **kwargs):
+        """z [N, embed_dim, h, w] -> [N, 3, 8h, 8w] fp16.  Like the reference, post_quant_conv runs only when no kwargs
+        are given; the plain Decoder takes none (ae_modules.py:538), so decode(z) is its one form."""
+        if kwargs:
+            raise NotImplementedError("the plain AutoencoderKL decoder takes no decode kwargs (ref_context / "
+                                      "timesteps belong to AutoencoderKL_Dualref)")
+        from . import runtime
+        return self.decoder_engine().decode(z.float(), executor=runtime.TEST_EXECUTOR).clone()
+
+    def decoder_engine(self):
+        """The PlainDecoderEngine decode() runs on (built on first use).  Its decode() returns a view of the plan's
+        static output buffer, valid until the next decode of the same geometry: for callers that consume it in place."""
+        from . import runtime
+        from .vae_engine import PlainDecoderEngine
+        return PlainDecoderEngine.cached(self, "_dec_engine", runtime.TEST_EXECUTOR)
+
+
+class AutoencoderKL_Dualref(AutoencoderKL):
+    def _make_decoder(self, dd):
+        return modules.VideoDecoder(**dd)
 
     def decode(self, z, **kwargs):
         """kwargs: ref_context (5 maps [b, C, 2, H, W]) and timesteps, as decode_core passes them."""
@@ -150,11 +170,6 @@ class AutoencoderKL(nn.Module):
         from . import runtime
         from .vae_engine import DecoderEngine
         return DecoderEngine.cached(self, "_dec_engine", runtime.TEST_EXECUTOR, module=self.decoder)
-
-
-class AutoencoderKL_Dualref(AutoencoderKL):
-    def _make_decoder(self, dd):
-        return modules.VideoDecoder(**dd)
 
 
 class LatentVisualDiffusion(nn.Module):
@@ -298,16 +313,20 @@ class LatentVisualDiffusion(nn.Module):
             b, _, t, _, _ = z.shape
             z = z.permute(0, 2, 1, 3, 4).reshape(b * t, z.shape[1], *z.shape[3:])
         z = 1.0 / self.scale_factor * z
+        video_decoder = isinstance(self.first_stage_model.decoder, modules.VideoDecoder)
         if not self.perframe_ae:
-            raise NotImplementedError("VideoDecoder needs the chunked (perframe_ae=True) path")
-        n = self.en_and_decode_n_samples_a_time or self.temporal_length
-        outs = []
-        for i in range(0, z.shape[0], n):
-            chunk = z[i:i + n]
-            kw = dict(kwargs)
-            kw["timesteps"] = chunk.shape[0]
-            outs.append(self.first_stage_model.decode(chunk, **kw))
-        out = torch.cat(outs, dim=0)
+            if video_decoder:
+                raise NotImplementedError("VideoDecoder needs the chunked (perframe_ae=True) path")
+            out = self.first_stage_model.decode(z, **kwargs)
+        else:
+            n = self.en_and_decode_n_samples_a_time or self.temporal_length
+            outs = []
+            for i in range(0, z.shape[0], n):
+                chunk = z[i:i + n]
+                # ddpm3d.py:664-667: only a VideoDecoder gets the caller's kwargs plus timesteps; any other decoder none
+                kw = dict(kwargs, timesteps=chunk.shape[0]) if video_decoder else {}
+                outs.append(self.first_stage_model.decode(chunk, **kw))
+            out = torch.cat(outs, dim=0)
         if five_d:
             out = out.reshape(b, t, *out.shape[1:]).permute(0, 2, 1, 3, 4)
         return out

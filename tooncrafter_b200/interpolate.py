@@ -3,10 +3,16 @@
     python -m tooncrafter_b200.interpolate --config configs/inference_512_v1.0.yaml --ckpt model.ckpt \
         --frames a.png b.png c.png --prompt "an anime scene" --out results/storyboard
 
+With a single --frames image the image is animated instead (ToonCrafterPipeline.animate, image-to-video):
+
+    python -m tooncrafter_b200.interpolate --config configs/training_1024_v1.0/config.yaml --ckpt model.ckpt \
+        --frames still.png --height 576 --width 1024 --out results/clip
+
 Writes DIR/frame_%04d.png, DIR/video.npy (uint8 [F, H, W, 3]) and, when OpenCV can open an mp4 writer,
 DIR/video.mp4.  The sampling defaults are those of the reference's scripts/run.sh.
 
-The config is the reference-style YAML (read with PyYAML).  Its two OpenCLIP conditioning targets
+The config is the reference-style YAML (read with PyYAML; only its `model:` section is used, so the training
+configs, whose first stage is the plain AutoencoderKL, work as well).  Its two OpenCLIP conditioning targets
 (lvdm.modules.encoders.condition.FrozenOpenCLIP*) are pointed at this repository's classes unless
 --keep-config-targets is given.  --synthetic-weights replaces the checkpoint by seeded synthetic weights (smoke runs).
 """
@@ -33,7 +39,8 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--synthetic-weights", action="store_true", help="seeded synthetic weights instead of --ckpt")
     ap.add_argument("--keep-config-targets", action="store_true",
                     help="keep the YAML's OpenCLIP targets instead of this repository's classes")
-    ap.add_argument("--frames", nargs="+", required=True, help="K >= 2 keyframe images, in order")
+    ap.add_argument("--frames", nargs="+", required=True,
+                    help="K >= 2 keyframe images, in order; one image: animate it")
     ap.add_argument("--prompt", default="", help="prompt of every segment")
     ap.add_argument("--prompts-file", default=None, help="one prompt per segment, one per non-empty line")
     ap.add_argument("--out", required=True, help="output directory")
@@ -46,7 +53,8 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--frame-stride", type=int, default=10, help="fs conditioning (smaller: larger motion)")
     ap.add_argument("--guidance-rescale", type=float, default=0.7)
     ap.add_argument("--timestep-spacing", default="uniform_trailing")
-    ap.add_argument("--segments-per-batch", type=int, default=4)
+    ap.add_argument("--segments-per-batch", type=int, default=None,
+                    help="segments sampled together (default: 4 at 320x512, 1 at 576x1024)")
     ap.add_argument("--loop", action="store_true", help="add a closing segment from the last keyframe to the first")
     ap.add_argument("--seed", type=int, default=123)
     ap.add_argument("--fps", type=int, default=8, help="frame rate of the mp4")
@@ -142,15 +150,22 @@ def main(argv=None) -> int:
         model = model.to(dev).eval()
     model.perframe_ae = True
     frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
-    n_seg = len(frames) if args.loop else len(frames) - 1
-    video = ToonCrafterPipeline(model).interpolate(
-        frames, prompts=read_prompts(args, n_seg), steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta,
-        fs=args.frame_stride, guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing,
-        cfg_img=args.cfg_img, loop=args.loop, seed=args.seed, size=(args.height, args.width),
-        segments_per_batch=args.segments_per_batch)
+    pipe = ToonCrafterPipeline(model)
+    common = dict(steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta, fs=args.frame_stride,
+                  guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing, cfg_img=args.cfg_img,
+                  seed=args.seed, size=(args.height, args.width))
+    if len(frames) == 1:
+        if args.loop:
+            raise SystemExit("--loop needs at least two keyframes")
+        video = pipe.animate(frames[0], prompt=read_prompts(args, 1), **common)
+    else:
+        n_seg = len(frames) if args.loop else len(frames) - 1
+        video = pipe.interpolate(frames, prompts=read_prompts(args, n_seg), loop=args.loop,
+                                 segments_per_batch=args.segments_per_batch, **common)
     v = video.cpu().numpy()
     write_video(v, args.out, args.fps)
-    print(f"{len(frames)} keyframes -> {v.shape[0]} frames of {v.shape[1]}x{v.shape[2]} in {args.out}")
+    print(f"{len(frames)} {'image' if len(frames) == 1 else 'keyframes'} -> {v.shape[0]} frames of "
+          f"{v.shape[1]}x{v.shape[2]} in {args.out}")
     return 0
 
 

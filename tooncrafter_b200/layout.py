@@ -158,6 +158,39 @@ def decoder_layout(dd) -> DecoderLayout:
     return lay
 
 
+def plain_decoder_layout(dd) -> DecoderLayout:
+    """lvdm/modules/networks/ae_modules.py:478-536 (the per-frame AutoencoderKL Decoder): num_res_blocks + 1
+    ResnetBlocks per level, an upsampling conv on every level but 0, no reference-frame refinement.  Only the options
+    the reference's configs use are accepted."""
+    if list(_get(dd, "attn_resolutions", [])):
+        raise NotImplementedError("Decoder with attn_resolutions != [] is outside the supported hot path")
+    for flag in ("give_pre_end", "tanh_out", "use_linear_attn"):
+        if _get(dd, flag, False):
+            raise NotImplementedError(f"Decoder option {flag}=True is outside the supported hot path")
+    if _get(dd, "attn_type", "vanilla") != "vanilla":
+        raise NotImplementedError(f"Decoder attn_type={_get(dd, 'attn_type')!r} is outside the supported hot path")
+    if not _get(dd, "resamp_with_conv", True):
+        raise NotImplementedError("Decoder resamp_with_conv=False is outside the supported hot path")
+    ch = _get(dd, "ch")
+    ch_mult = list(_get(dd, "ch_mult"))
+    nres = _get(dd, "num_res_blocks")
+    nlev = len(ch_mult)
+    block_in = ch * ch_mult[-1]
+    lay = DecoderLayout(z_channels=_get(dd, "z_channels"), ch=ch, out_ch=_get(dd, "out_ch"), num_resolutions=nlev,
+                        num_res_blocks=nres, block_in=block_in)
+    levels = [None] * nlev
+    cur = block_in
+    for i_level in reversed(range(nlev)):
+        cout = ch * ch_mult[i_level]
+        blocks = []
+        for _ in range(nres + 1):
+            blocks.append((cur, cout))
+            cur = cout
+        levels[i_level] = dict(blocks=blocks, upsample=(i_level != 0), channels=cur)
+    lay.levels = levels
+    return lay
+
+
 @dataclass
 class EncoderLayout:
     in_channels: int

@@ -6,7 +6,7 @@ included), but contain no arithmetic: `forward` hands the tensors to the CUDA en
 
 Reference constructors mirrored (names/shapes only): lvdm/modules/networks/openaimodel3d.py:109-195,239-270,
 311-546; lvdm/modules/attention.py:42-78,212-229,249-291,313-363,415-439; lvdm/models/autoencoder_dualref.py
-:35-70,145-170,256-262,343-349,371-487,846-880,914-927; lvdm/modules/networks/ae_modules.py:92-108,366-430;
+:35-70,145-170,256-262,343-349,371-487,846-880,914-927; lvdm/modules/networks/ae_modules.py:92-108,366-430,478-536;
 lvdm/modules/attention_svd.py:347-371.
 """
 from __future__ import annotations
@@ -14,7 +14,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from .layout import Layer, decoder_layout, encoder_layout, unet_layout
+from .layout import Layer, decoder_layout, encoder_layout, plain_decoder_layout, unet_layout
 
 
 class Node(nn.Module):
@@ -236,6 +236,27 @@ class VideoDecoder(nn.Module):
         conv_out = nn.Conv2d(c0, lay.out_ch, 3, padding=1)
         conv_out.add_module("time_mix_conv", nn.Conv3d(lay.out_ch, lay.out_ch, (3, 1, 1), padding=(1, 0, 0)))
         self.conv_out = conv_out
+
+
+class Decoder(nn.Module):
+    """Parameter holder for lvdm.modules.networks.ae_modules.Decoder, the per-frame 2-D decoder of the plain
+    AutoencoderKL (attn_resolutions = [])."""
+
+    def __init__(self, **ddconfig):
+        super().__init__()
+        lay = self.layout = plain_decoder_layout(ddconfig)
+        self.conv_in = nn.Conv2d(lay.z_channels, lay.block_in, 3, padding=1)
+        self.mid = Node(block_1=_vae_resnet(lay.block_in, lay.block_in), attn_1=_attn_block(lay.block_in),
+                        block_2=_vae_resnet(lay.block_in, lay.block_in))
+        self.up = Node()
+        for i, lv in enumerate(lay.levels):
+            up = Node(block=_numbered({j: _vae_resnet(a, b) for j, (a, b) in enumerate(lv["blocks"])}), attn=Node())
+            if lv["upsample"]:
+                up.put("upsample", Node(conv=nn.Conv2d(lv["channels"], lv["channels"], 3, padding=1)))
+            self.up.put(i, up)
+        c0 = lay.levels[0]["channels"]
+        self.norm_out = _gn(c0, 1e-6)
+        self.conv_out = nn.Conv2d(c0, lay.out_ch, 3, padding=1)
 
 
 class Encoder(nn.Module):

@@ -144,11 +144,16 @@ def last_gemm_config() -> dict:
 
 
 _GN_WS = {}
+_GN_WS_RETIRED = []
 
 
 def _gn_ws(device, n_floats: int) -> torch.Tensor:
+    """Per-device statistics scratch of tc_groupnorm, grown on demand.  A grown-out workspace is retired, never freed:
+    CUDA graphs captured while it was current keep its address and still write to it when they are replayed."""
     ws = _GN_WS.get(device)
     if ws is None or ws.numel() < n_floats:
+        if ws is not None:
+            _GN_WS_RETIRED.append(ws)
         ws = torch.empty(max(n_floats, 1 << 20), dtype=torch.float32, device=device)
         _GN_WS[device] = ws
     return ws

@@ -14,7 +14,8 @@ Per call:
   * ONE image-tower pass over the first keyframe of every segment plus the zero image, ONE text-tower pass over the
     distinct prompts plus "" (inference.py:186-216);
   * the segments as the batch rows of one fused DDIM sample() per group of `segments_per_batch`;
-  * per segment the T = 16 and T = 14 decodes (inference.py:262-270), read in place by one tc_video_u8 launch that
+  * per segment the T = 16 and T = 14 decodes (inference.py:262-270; one decode with a plain first stage, see below),
+    read in place by one tc_video_u8 launch that
     applies the middle-frame splice and the uint8 conversion of the save path and writes the segment's frames into
     the joined video at frame (T-1)*k.
 
@@ -26,16 +27,23 @@ So segment k of a K-keyframe run is the same computation as a 2-keyframe run on 
 Seam rule: neighbouring segments share a keyframe; the earlier segment's last frame is kept and the later segment's
 frame 0 is dropped.  With `loop`, the closing segment's last frame (keyframe 0 again) is dropped as well, so the
 video has (T-1)*S + 1 frames, or (T-1)*K with `loop`.
+
+`ToonCrafterPipeline.animate` is the same glue for one image (image_guided_synthesis with interp=False): one segment
+whose c_concat is the image's latent repeated over the T frames.
+
+First stage: with the dual-reference AutoencoderKL_Dualref each segment is decoded twice (T = 16 and T = 14, then
+spliced, as above).  The plain AutoencoderKL of the DynamiCrafter / training configs decodes every frame on its own, so
+each segment is decoded once, without reference maps, and tc_video_u8 runs without a splice.
 """
 from __future__ import annotations
 
-from typing import Sequence, Union
+from typing import Optional, Sequence, Union
 
 import numpy as np
 import torch
 
 from . import ops, runtime
-from .modules import clip_tokenize
+from .modules import VideoDecoder, clip_tokenize
 from .sampler import DDIMSampler, DDIMSamplerMultiCond
 
 
@@ -60,6 +68,14 @@ def preprocess(keyframes, size=(320, 512), device="cpu") -> torch.Tensor:
             t = TF.center_crop(t, list(size))
         out.append(t)
     return torch.stack(out).float().div(255).sub(0.5).div(0.5)
+
+
+def default_segments_per_batch(size) -> int:
+    """Segments sampled together by default: as many as keep the UNet program at the activation budget of 4 segments
+    at 320 x 512 (8 rows of a 40 x 64 latent, an arena of about 8 GB; it grows with rows x latent pixels).  At
+    576 x 1024 that is 1 segment: with 4 the UNet arena alone would take 28 GiB, and a default call after an animate
+    call (whose plans stay cached) no longer fits on an 80 GB H100."""
+    return max(1, (4 * 320 * 512) // (size[0] * size[1]))
 
 
 class ToonCrafterPipeline:
@@ -89,33 +105,69 @@ class ToonCrafterPipeline:
     def interpolate(self, keyframes, prompts: Union[str, Sequence[str], torch.Tensor] = "", steps: int = 50,
                     cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                     timestep_spacing: str = "uniform_trailing", cfg_img=None, loop: bool = False, seed: int = 123,
-                    size=(320, 512), segments_per_batch: int = 4, output: str = "uint8") -> torch.Tensor:
+                    size=(320, 512), segments_per_batch: Optional[int] = None, output: str = "uint8") -> torch.Tensor:
         """keyframes: K >= 2 uint8 RGB images (tensor [K, H, W, 3], ndarray, or a list of [H, W, 3] arrays of any
         size).  prompts: one string for every segment, a list of S strings, or token ids [S, 77] (strings other than
         "" need open_clip's tokenizer).  cfg_img not None: three-way guidance (DDIMSamplerMultiCond).  Defaults are
         those of the reference's scripts/run.sh.
 
+        segments_per_batch None: default_segments_per_batch(size), 4 at 320 x 512 and 1 at 576 x 1024.
+
         Returns uint8 [F, size[0], size[1], 3] on the model's device, F = (T-1)*S + 1 (or (T-1)*K with `loop`); with
         output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]]."""
+        if segments_per_batch is None:
+            segments_per_batch = default_segments_per_batch(size)
+        frames = self._preprocess(keyframes, size, output)
+        K = frames.shape[0]
+        if K < 2:
+            raise ValueError("interpolation needs at least two keyframes")
+        S = K if loop else K - 1
+        return self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, steps, cfg_scale,
+                              eta, fs, guidance_rescale, timestep_spacing, cfg_img, loop, seed, size,
+                              segments_per_batch, output)
+
+    @torch.no_grad()
+    def animate(self, image, prompt: Union[str, torch.Tensor] = "", steps: int = 50, cfg_scale: float = 7.5,
+                eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
+                timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
+                output: str = "uint8") -> torch.Tensor:
+        """One image -> one T-frame video: image_guided_synthesis with interp=False, loop=False (inference.py:
+        180-277; c_concat is the image's latent repeated over the T frames, :201-203), the image-to-video mode of
+        the DynamiCrafter checkpoints.  image: a uint8 [H, W, 3] RGB image of any size; prompt: a string or token
+        ids [1, 77].  The image's posterior noise comes from a CPU generator seeded `seed`, x_T and the DDIM step
+        noise from a generator on the model's device seeded `seed` (keyframe 0 / segment 0 of `interpolate`); a
+        dual-reference first stage gets the image's encoder maps as both reference frames.
+
+        Returns uint8 [T, size[0], size[1], 3] on the model's device; with output="float", the spliced video before
+        quantisation, float32 [3, T, size[0], size[1]]."""
+        frames = self._preprocess([image], size, output)
+        video = self._generate(frames, prompt, [0], [0], False, steps, cfg_scale, eta, fs, guidance_rescale,
+                               timestep_spacing, cfg_img, False, seed, size, 1, output)
+        return video[0] if output == "float" else video
+
+    def _preprocess(self, images, size, output) -> torch.Tensor:
+        """Argument checks shared by interpolate and animate, then preprocess() onto the model's device."""
         m = self.model
-        dev = m.device
         if output not in ("uint8", "float"):
             raise ValueError(f"output must be 'uint8' or 'float', got {output!r}")
         if size[0] % 16 or size[1] % 16:
             raise ValueError(f"size {tuple(size)} must be a multiple of 16")
         if m.model.conditioning_key != "hybrid":
-            raise NotImplementedError("keyframe interpolation needs the hybrid (concat + cross-attention) model")
+            raise NotImplementedError("image-conditioned synthesis needs the hybrid (concat + cross-attention) model")
         T = m.temporal_length
         if (m.en_and_decode_n_samples_a_time or T) < T:
             raise NotImplementedError("the pipeline decodes each segment's T frames in one call")
+        return preprocess(images, size, m.device)
+
+    def _generate(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
+                  timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output) -> torch.Tensor:
+        """S = len(first) segments; segment k runs from keyframe first[k] to keyframe last[k] (interp), or animates
+        keyframe first[k] (not interp)."""
+        m = self.model
+        dev = m.device
+        T = m.temporal_length
         ex = runtime.TEST_EXECUTOR
-        frames = preprocess(keyframes, size, dev)
-        K = frames.shape[0]
-        if K < 2:
-            raise ValueError("interpolation needs at least two keyframes")
-        S = K if loop else K - 1
-        first = list(range(S))
-        last = [(k + 1) % K for k in range(S)]
+        K, S = frames.shape[0], len(first)
 
         # conditioning: text over the distinct prompts + "", image over each segment's first keyframe + the zero image
         cond_emb, empty_emb = self._text(prompts, S)
@@ -135,15 +187,19 @@ class ToonCrafterPipeline:
                              for j in range(K)])
         z = m.get_first_stage_encoding(post, noise=noise)                           # [K, 4, h, w]
         h, w = z.shape[-2:]
-        c_concat = torch.zeros(S, z.shape[1], T, h, w, dtype=z.dtype, device=dev)
-        c_concat[:, :, 0] = z[first]
-        c_concat[:, :, -1] = z[last]
+        if interp:
+            c_concat = torch.zeros(S, z.shape[1], T, h, w, dtype=z.dtype, device=dev)
+            c_concat[:, :, 0] = z[first]
+            c_concat[:, :, -1] = z[last]
+        else:
+            c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
 
         F = (T - 1) * S + (0 if loop else 1)
         video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=dev) if output == "uint8" else
                  torch.empty(S, 3, T, size[0], size[1], dtype=torch.float32, device=dev))
         sampler = DDIMSampler(m) if cfg_img is None else DDIMSamplerMultiCond(m)
         dec = m.first_stage_model.decoder_engine()
+        dual_ref = isinstance(m.first_stage_model.decoder, VideoDecoder)
         keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
         for g0 in range(0, S, segments_per_batch):
             seg = list(range(g0, min(g0 + segments_per_batch, S)))
@@ -164,13 +220,22 @@ class ToonCrafterPipeline:
                                         timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale,
                                         noise_generators=gens, **extra)
             for i, k in enumerate(seg):
-                ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
                 lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
-                y16 = dec.decode(lat.float(), ref, executor=ex)                         # views of the plans' outputs
-                y14 = dec.decode(lat[keep].float(), ref, executor=ex)
+                if dual_ref:
+                    ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
+                    y16 = dec.decode(lat.float(), ref, executor=ex)                     # views of the plans' outputs
+                    y14 = dec.decode(lat[keep].float(), ref, executor=ex)
+                else:
+                    # A frame-independent decoder turns each latent into the same frame whichever chunk holds it, so
+                    # the reference's T - 2 pass is y16[keep] and the T - 2 decode is skipped.  For T >= 6 the two
+                    # spliced frames (keep[T/2-2], keep[T/2-1] = latents T/2-1, T/2) are the frames already in place:
+                    # no splice at all (tc_video_u8 with x14 = NULL).
+                    y16 = dec.decode(lat.float(), executor=ex)
+                    y14 = None if T >= 6 else y16[keep]
                 if output == "float":
                     v = y16.float()
-                    v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
+                    if y14 is not None:
+                        v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
                     video[k] = v.permute(1, 0, 2, 3)
                     continue
                 f_begin = 0 if k == 0 else 1

@@ -48,10 +48,28 @@ def fill_module_(module: torch.nn.Module, seed: int = 0, prefix: str = "") -> No
             p.copy_(synthetic_tensor(prefix + k, tuple(p.shape), seed).to(p.dtype))
 
 
-def synthetic_model(config, device, seed: int = 0) -> torch.nn.Module:
+FIRST_STAGE_TARGETS = {"plain": "lvdm.models.autoencoder.AutoencoderKL",
+                       "dualref": "lvdm.models.autoencoder.AutoencoderKL_Dualref"}
+
+
+def with_first_stage(config, first_stage: str):
+    """A copy of a LatentVisualDiffusion config whose first stage is the plain AutoencoderKL ("plain": the DynamiCrafter
+    and training configs) or AutoencoderKL_Dualref ("dualref": the ToonCrafter inference configs), same ddconfig."""
+    import copy
+    if first_stage not in FIRST_STAGE_TARGETS:
+        raise ValueError(f"first_stage must be one of {sorted(FIRST_STAGE_TARGETS)}, got {first_stage!r}")
+    cfg = copy.deepcopy(config)
+    cfg["params"]["first_stage_config"]["target"] = FIRST_STAGE_TARGETS[first_stage]
+    return cfg
+
+
+def synthetic_model(config, device, seed: int = 0, first_stage=None) -> torch.nn.Module:
     """instantiate_from_config(config) with the weights fill_module_(model, seed) gives, built straight on `device`
-    (meta skeleton, each tensor drawn on the host and copied over), so a full-size model needs no host-side copy."""
+    (meta skeleton, each tensor drawn on the host and copied over), so a full-size model needs no host-side copy.
+    first_stage "plain" / "dualref" replaces the config's first-stage class (with_first_stage)."""
     from . import diffusion, modules
+    if first_stage is not None:
+        config = with_first_stage(config, first_stage)
     with torch.device("meta"):
         skeleton = diffusion.instantiate_from_config(config)
     m = skeleton.to_empty(device=device)

@@ -1,4 +1,6 @@
-"""CUDA execution engine for the dual-reference video decoder (AutoencoderKL_Dualref / VideoDecoder).
+"""CUDA execution engines for the first stage: the dual-reference video decoder (AutoencoderKL_Dualref /
+VideoDecoder, `DecoderEngine`), the plain per-frame decoder of AutoencoderKL (`PlainDecoderEngine`) and the shared
+encoder (`EncoderEngine`).
 
 Reference semantics restated (paths relative to /root/reference):
   Decoder.forward                     lvdm/models/autoencoder_dualref.py:489-527
@@ -239,6 +241,115 @@ class DecoderEngine(Engine):
         plan.z_in.copy_(z.reshape(plan.z_in.shape))
         self._execute(plan.main, executor, self.use_graph)
         return plan.y_out.reshape(T, self.lay.out_ch, plan.y_out.shape[-2], plan.y_out.shape[-1])
+
+
+class PlainDecoderEngine(Engine):
+    """AutoencoderKL.decode(z) without kwargs for the plain per-frame Decoder: post_quant_conv + Decoder.forward.
+
+    Reference: lvdm/models/autoencoder.py:112-116 (post_quant_conv), lvdm/modules/networks/ae_modules.py:538-575
+    (Decoder.forward), :153-213 (ResnetBlock, temb None), :28-75 (AttnBlock), :78-89 (Upsample, nearest + 3x3 conv).
+    Every frame is decoded independently, so one plan serves any number of frames N and chunking does not change the
+    result."""
+
+    def __init__(self, ae: nn.Module, device=None, arena_bytes: int = 0, use_graph: bool = True,
+                 plan_only: bool = False):
+        super().__init__(ae, device, use_graph, plan_only)
+        self.lay: DecoderLayout = ae.decoder.layout
+        self.arena_bytes = arena_bytes
+        self._pack(ae)
+
+    @staticmethod
+    def _weights(ae):
+        return (ae.decoder, ae.post_quant_conv)
+
+    def _pack(self, ae):
+        dev, lay, d = self.dev, self.lay, ae.decoder
+        self.cpad_in = (lay.z_channels + 63) // 64 * 64
+        pq = ae.post_quant_conv.weight.detach()
+        self.p_pq = _P(w=_h(torch.nn.functional.pad(pq.reshape(pq.shape[0], -1), (0, self.cpad_in - pq.shape[1])), dev),
+                       b=_f(ae.post_quant_conv.bias, dev))
+        self.p_conv_in = _P(w=pack_conv(d.conv_in.weight, dev, self.cpad_in), b=_f(d.conv_in.bias, dev))
+        self.p_mid1, self.p_mid2 = pack_vae_resnet(d.mid.block_1, dev), pack_vae_resnet(d.mid.block_2, dev)
+        self.p_attn = pack_mid_attention(d.mid.attn_1, lay.block_in, dev)
+        self.p_levels: List[_P] = []
+        for i, lv in enumerate(lay.levels):
+            up = d.up[i]
+            p = _P(blocks=[pack_vae_resnet(up.block[j], dev) for j in range(len(lv["blocks"]))], upsample=lv["upsample"])
+            if lv["upsample"]:
+                p.up_w, p.up_b = pack_conv(up.upsample.conv.weight, dev), _f(up.upsample.conv.bias, dev)
+            self.p_levels.append(p)
+        self.p_final = _P(norm=pack_norm(d.norm_out, dev), out_w=pack_conv(d.conv_out.weight, dev),
+                          out_b=_f(d.conv_out.bias, dev))
+
+    def arena_size(self, N: int, h: int, w: int) -> int:
+        """Bytes of activation arena a plan for N frames of an h x w latent takes: 3.5 maps of the widest
+        full-resolution activation (level 1's channels after its upsampling; the program peaks at 3.25 of them in
+        level 0's first ResnetBlock) plus 64 MiB of slack for the low-resolution levels."""
+        lay = self.lay
+        nlev = lay.num_resolutions
+        H0, W0 = h * 2 ** (nlev - 1), w * 2 ** (nlev - 1)
+        widest = max(lv["channels"] for lv in lay.levels[:2])
+        return self.arena_bytes or int(3.5 * N * H0 * W0 * widest * 2 + (64 << 20))
+
+    def _build(self, N: int, h: int, w: int):
+        lay, dev = self.lay, self.dev
+        arena = Arena(self.arena_size(N, h, w), dev)
+        main = Program()
+        bld = Builder(arena, main)
+        plan = _P(N=N, h=h, w=w, arena=arena, main=main)
+        plan.z_in = torch.zeros(N, lay.z_channels, 1, h, w, dtype=torch.float32, device=dev)
+        # the padding channels of both buffers stay zero: conv_in and post_quant_conv read all cpad_in of them
+        z_cl = torch.zeros(N * h * w * self.cpad_in, dtype=torch.float16, device=dev)
+        pq_t = torch.zeros(N * h * w * self.cpad_in, dtype=torch.float16, device=dev)
+        main.add(ops.ncthw_to_cl, plan.z_in, z_cl, B=N, C_=lay.z_channels, T=1, H=h, W=w, Cpad=self.cpad_in, coff=0,
+                 scale=1.0)
+        pq = Act(pq_t, N, h, w, self.cpad_in, self.cpad_in)
+        linear(bld, Act(z_cl, N, h, w, self.cpad_in, self.cpad_in), self.p_pq.w, pq, bias=self.p_pq.b,
+               n_cols=lay.z_channels)
+        cur = bld.act(N, h, w, lay.block_in)
+        gemm(bld, pq, self.p_conv_in.w, ops.TAPS_3x3, cur, bias=self.p_conv_in.b)
+
+        nxt = bld.act(N, h, w, lay.block_in)
+        resblock(bld, self.p_mid1, cur, nxt); cur.free(); cur = nxt
+        nxt = bld.act(N, h, w, lay.block_in)
+        mid_attention(bld, self.p_attn, cur, nxt); cur.free(); cur = nxt
+        nxt = bld.act(N, h, w, lay.block_in)
+        resblock(bld, self.p_mid2, cur, nxt); cur.free(); cur = nxt
+        for i in reversed(range(lay.num_resolutions)):
+            p = self.p_levels[i]
+            for rb in p.blocks:
+                nxt = bld.act(N, cur.H, cur.W, rb.cout)
+                resblock(bld, rb, cur, nxt); cur.free(); cur = nxt
+            if p.upsample:
+                up = bld.act(N, 2 * cur.H, 2 * cur.W, cur.C)
+                bld.op(ops.upsample2x, cur.t, up.t, N=N, H=cur.H, W=cur.W, C_=cur.C)
+                cur.free()
+                nxt = bld.act(N, up.H, up.W, up.C)
+                gemm(bld, up, p.up_w, ops.TAPS_3x3, nxt, bias=p.up_b)
+                up.free()
+                cur = nxt
+        pf = self.p_final
+        g = bld.act(N, cur.H, cur.W, cur.C)
+        groupnorm(bld, cur, g, pf.norm, silu=True)
+        cur.free()
+        # conv_out (C -> out_ch) into a 64-channel buffer, read back as NCHW
+        Hf, Wf = g.H, g.W
+        co_t = torch.zeros(N * Hf * Wf * 64, dtype=torch.float16, device=dev)
+        gemm(bld, g, pf.out_w, ops.TAPS_3x3, Act(co_t, N, Hf, Wf, 64, 64), bias=pf.out_b, n_cols=lay.out_ch)
+        g.free()
+        plan.y_out = torch.zeros(N, lay.out_ch, 1, Hf, Wf, dtype=torch.float16, device=dev)
+        main.add(ops.cl_to_ncthw, co_t, plan.y_out, B=N, C_=lay.out_ch, T=1, H=Hf, W=Wf, ldx=64)
+        return plan
+
+    @torch.no_grad()
+    def decode(self, z: torch.Tensor, executor=None) -> torch.Tensor:
+        """z [N, z_channels, h, w] (already divided by scale_factor) -> [N, 3, 8h, 8w] fp16, a view of the plan's
+        static output buffer (valid until the next decode of the same geometry)."""
+        N, _, h, w = z.shape
+        plan = self.plan_for(N, h, w)
+        plan.z_in.copy_(z.reshape(plan.z_in.shape))
+        self._execute(plan.main, executor, self.use_graph)
+        return plan.y_out.reshape(N, self.lay.out_ch, plan.y_out.shape[-2], plan.y_out.shape[-1])
 
 
 class EncoderEngine(Engine):
