@@ -16,11 +16,22 @@ not depend on the step count), and the first-stage decode of 16 latents, plain a
 events, 10 replays after a warm-up):
 
     python scripts/bench_pipeline.py --animate --first-stage plain --size 576 1024
+
+--gpus N measures ToonCrafterPipeline sharded over N GPUs, one process per GPU under torchrun (--gpus 1: the same
+workload on one GPU, without torchrun): a K = 5 interpolate() at --size, or with --animate one animate() call, with
+--latency-mode one clip per GPU pair.  Warm-up at DDIM-2, then `--reps` timed calls, each between a barrier and a
+device synchronise; the time reported is the maximum over ranks.
+
+    python scripts/bench_pipeline.py --gpus 1
+    torchrun --nproc-per-node 2 scripts/bench_pipeline.py --gpus 2 [--latency-mode]
+    torchrun --nproc-per-node 2 scripts/bench_pipeline.py --gpus 2 --latency-mode --animate --first-stage plain \
+        --size 576 1024
 """
 from __future__ import annotations
 
 import argparse
 import json
+import os
 import subprocess
 import sys
 import time
@@ -141,6 +152,44 @@ def bench_animate(args, model, info, build_s, decode16):
     return 0
 
 
+def bench_sharded(args, model, info, build_s, group):
+    """--gpus N: K = 5 interpolate (or animate) sharded over `group` (None: one GPU); see the module docstring."""
+    import torch.distributed as dist
+
+    from tooncrafter_b200.distributed import max_over_ranks
+    from tooncrafter_b200.pipeline import ToonCrafterPipeline
+    size = tuple(args.size)
+    pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
+    g = torch.Generator().manual_seed(0)
+    kf = (torch.rand(5, size[0], size[1], 3, generator=g) * 255).to(torch.uint8)
+    if args.animate:
+        fn, frames, what = (lambda st: pipe.animate(kf[0], steps=st, seed=123, size=size)), 16, "animate"
+    else:
+        fn, frames, what = (lambda st: pipe.interpolate(kf, steps=st, seed=123, size=size)), 15 * 4 + 1, "K=5"
+    fn(2)
+    times = []
+    for _ in range(args.reps):
+        torch.cuda.synchronize()
+        if group is not None:
+            dist.barrier(group)
+        t = time.perf_counter()
+        fn(args.ddim_steps)
+        torch.cuda.synchronize()
+        times.append(max_over_ranks(time.perf_counter() - t, model.device))
+    if group is not None and dist.get_rank() != 0:
+        return 0
+    best = min(times)
+    out = dict(metric="%s %s: seconds per video over %d GPU%s (%dx%d, DDIM-%d, CFG 7.5, eta 1, synthetic weights, %s "
+               "first stage)" % (what, "latency mode" if args.latency_mode else "sharded", args.gpus,
+                                 "s" if args.gpus > 1 else "", size[0], size[1], args.ddim_steps, args.first_stage),
+               gpu=info, gpus=args.gpus, latency_mode=args.latency_mode, reps=args.reps, model_build_s=build_s,
+               frames=frames, sec_per_video=best, frames_per_s=frames / best, all_s=[round(x, 3) for x in times],
+               note="sec_per_video = best of the timed reps; each rep is the maximum over ranks of a host clock "
+                    "started after a barrier and stopped after a device synchronise")
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reps", type=int, default=2)
@@ -149,22 +198,41 @@ def main():
                     help="AutoencoderKL_Dualref (ToonCrafter) or the plain AutoencoderKL (DynamiCrafter / training configs)")
     ap.add_argument("--size", type=int, nargs=2, default=(320, 512), metavar=("H", "W"))
     ap.add_argument("--animate", action="store_true", help="measure animate and K = 2 interpolation (docstring)")
+    ap.add_argument("--gpus", type=int, default=None,
+                    help="measure the pipeline sharded over N GPUs, under torchrun when N > 1 (docstring)")
+    ap.add_argument("--latency-mode", action="store_true", help="with --gpus: one clip per GPU pair")
     args = ap.parse_args()
     from tooncrafter_b200 import synthetic
     from tooncrafter_b200.pipeline import ToonCrafterPipeline
     if not torch.cuda.is_available():
         raise SystemExit("bench_pipeline.py measures the GPU; no CUDA device found")
-    dev = torch.device("cuda")
+    dev, group = torch.device("cuda"), None
+    if args.gpus is not None and args.gpus > 1:
+        import torch.distributed as dist
+        if int(os.environ.get("WORLD_SIZE", "1")) != args.gpus:
+            raise SystemExit(f"--gpus {args.gpus}: run under torchrun --nproc-per-node {args.gpus}")
+        dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
+        torch.cuda.set_device(dev)
+        dist.init_process_group("nccl", device_id=dev)
+        group = dist.group.WORLD
+    elif args.latency_mode:
+        raise SystemExit("--latency-mode pairs GPUs: give --gpus N with an even N, under torchrun")
     info = gpu_info()
     print(f"GPU: {info['name']}, power limit {info['power_limit']}", flush=True)
     torch.backends.cuda.matmul.allow_tf32 = False
     size = tuple(args.size)
-    decode16 = decode_ms(size) if args.animate else None       # before the model: the two decoders' plans alone
+    decode16 = decode_ms(size) if args.animate and args.gpus is None else None   # before the model: the decoders alone
     torch.cuda.empty_cache()
     t0 = time.perf_counter()
     model = synthetic.synthetic_model(full_pipeline_config(size), dev, first_stage=args.first_stage)
     model.perframe_ae = True
     build_s = time.perf_counter() - t0
+    if args.gpus is not None:
+        try:
+            return bench_sharded(args, model, info, build_s, group)
+        finally:
+            if group is not None:
+                torch.distributed.destroy_process_group()
     if args.animate:
         return bench_animate(args, model, info, build_s, decode16)
     pipe = ToonCrafterPipeline(model)

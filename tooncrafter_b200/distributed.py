@@ -69,18 +69,20 @@ def max_over_ranks(value: float, device="cpu") -> float:
     return float(t.item())
 
 
-def latency_pairs():
-    """Process groups of adjacent rank pairs (0,1), (2,3), ...; returns (group of this rank, pair index, rank in pair).
-    Every rank must call this (new_group is collective).  World size must be even."""
-    world, rank = dist.get_world_size(), dist.get_rank()
-    if world % 2:
+def latency_pairs(group=None):
+    """Process groups of adjacent rank pairs (0,1), (2,3), ... of `group` (default: the world); returns (group of this
+    rank, pair index, rank in pair).  Every rank of the world must call this (new_group is collective).  The size of
+    `group` must be even."""
+    ranks = list(range(dist.get_world_size())) if group is None else dist.get_process_group_ranks(group)
+    if len(ranks) % 2:
         raise ValueError("latency mode pairs GPUs: the world size must be even")
+    me = ranks.index(dist.get_rank())
     mine = None
-    for p in range(world // 2):
-        g = dist.new_group(ranks=[2 * p, 2 * p + 1])
-        if rank // 2 == p:
+    for p in range(len(ranks) // 2):
+        g = dist.new_group(ranks=ranks[2 * p:2 * p + 2])
+        if me // 2 == p:
             mine = g
-    return mine, rank // 2, rank % 2
+    return mine, me // 2, me % 2
 
 
 def _device_collectives(group) -> bool:
@@ -108,11 +110,15 @@ def pair_all_gather(out: torch.Tensor, inp: torch.Tensor, group) -> None:
     out.copy_(torch.cat(parts, 0))
 
 
-def sync_pair_state(x: torch.Tensor, group) -> None:
+def sync_pair_state(x: torch.Tensor, group, rng_state: bool = True) -> None:
     """Make the start latent and the CUDA RNG stream of a latency pair identical (pair-rank 0 wins), so that both ranks
-    draw the same per-step noise (ddim.py:273) and apply the same update."""
+    draw the same per-step noise (ddim.py:273) and apply the same update.  rng_state=False: the start latent only, for
+    a sampler whose rows draw their noise from per-row generators seeded alike on both ranks (the global RNG is then
+    not used, and is left alone)."""
     src = dist.get_global_rank(group, 0)
     pair_broadcast(x, src, group)
+    if not rng_state:
+        return
     state = torch.cuda.get_rng_state(x.device)              # a CPU byte tensor
     if _device_collectives(group):
         dstate = state.to(x.device)
@@ -121,3 +127,12 @@ def sync_pair_state(x: torch.Tensor, group) -> None:
     else:
         dist.broadcast(state, src=src, group=group)
     torch.cuda.set_rng_state(state, x.device)
+
+
+def broadcast_blocks(t: torch.Tensor, blocks, group) -> None:
+    """Assemble `t` on every rank of `group` from contiguous blocks along dim 0: blocks = [(src, begin, end), ...],
+    t[begin:end] of global rank `src` is copied to every other rank.  One broadcast per non-empty block, so blocks may
+    differ in size; device tensors go over NCCL directly, anything else through host memory (pair_broadcast)."""
+    for src, begin, end in blocks:
+        if end > begin:
+            pair_broadcast(t[begin:end], src, group)

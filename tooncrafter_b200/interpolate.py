@@ -11,6 +11,12 @@ With a single --frames image the image is animated instead (ToonCrafterPipeline.
 Writes DIR/frame_%04d.png, DIR/video.npy (uint8 [F, H, W, 3]) and, when OpenCV can open an mp4 writer,
 DIR/video.mp4.  The sampling defaults are those of the reference's scripts/run.sh.
 
+Under torchrun (WORLD_SIZE > 1) every process drives the GPU LOCAL_RANK over NCCL, builds the model (the checkpoint,
+or the same synthetic seed) and the segments are sharded over the processes (ToonCrafterPipeline's `group`);
+--latency-mode shards them over GPU pairs instead, one guidance branch per GPU.  Rank 0 writes the outputs:
+
+    torchrun --nproc-per-node 8 -m tooncrafter_b200.interpolate --config ... --frames a.png b.png c.png --out DIR
+
 The config is the reference-style YAML (read with PyYAML; only its `model:` section is used, so the training
 configs, whose first stage is the plain AutoencoderKL, work as well).  Its two OpenCLIP conditioning targets
 (lvdm.modules.encoders.condition.FrozenOpenCLIP*) are pointed at this repository's classes unless
@@ -57,6 +63,8 @@ def get_parser() -> argparse.ArgumentParser:
                     help="segments sampled together (default: 4 at 320x512, 1 at 576x1024)")
     ap.add_argument("--loop", action="store_true", help="add a closing segment from the last keyframe to the first")
     ap.add_argument("--seed", type=int, default=123)
+    ap.add_argument("--latency-mode", action="store_true",
+                    help="under torchrun: one clip per GPU pair, one guidance branch per GPU (even world size)")
     ap.add_argument("--fps", type=int, default=8, help="frame rate of the mp4")
     return ap
 
@@ -134,14 +142,30 @@ def main(argv=None) -> int:
     args = get_parser().parse_args(argv)
     if not args.synthetic_weights and args.ckpt is None:
         raise SystemExit("give --ckpt, or --synthetic-weights for a run without a checkpoint")
+    cfg = load_model_config(args.config, args.keep_config_targets)
+    if not torch.cuda.is_available():
+        raise SystemExit("a CUDA device is required")
+    world = int(os.environ.get("WORLD_SIZE", "1"))
+    if args.latency_mode and world == 1:
+        raise SystemExit("--latency-mode pairs GPUs: run under torchrun with an even number of processes")
+    if world == 1:
+        return run(args, cfg, torch.device("cuda"), None)
+    import torch.distributed as dist
+    dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", "0")))
+    torch.cuda.set_device(dev)
+    dist.init_process_group("nccl", device_id=dev)
+    try:
+        return run(args, cfg, dev, dist.group.WORLD)
+    finally:
+        dist.destroy_process_group()
+
+
+def run(args, cfg, dev, group) -> int:
+    """Build the model on `dev`, make the video (sharded over `group` when given) and write it from rank 0."""
     from PIL import Image
 
     from . import diffusion, synthetic
     from .pipeline import ToonCrafterPipeline
-    cfg = load_model_config(args.config, args.keep_config_targets)
-    if not torch.cuda.is_available():
-        raise SystemExit("a CUDA device is required")
-    dev = torch.device("cuda")
     if args.synthetic_weights:
         model = synthetic.synthetic_model(cfg, dev, seed=0)
     else:
@@ -150,7 +174,7 @@ def main(argv=None) -> int:
         model = model.to(dev).eval()
     model.perframe_ae = True
     frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
-    pipe = ToonCrafterPipeline(model)
+    pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
     common = dict(steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta, fs=args.frame_stride,
                   guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing, cfg_img=args.cfg_img,
                   seed=args.seed, size=(args.height, args.width))
@@ -162,6 +186,8 @@ def main(argv=None) -> int:
         n_seg = len(frames) if args.loop else len(frames) - 1
         video = pipe.interpolate(frames, prompts=read_prompts(args, n_seg), loop=args.loop,
                                  segments_per_batch=args.segments_per_batch, **common)
+    if group is not None and torch.distributed.get_rank() != 0:
+        return 0
     v = video.cpu().numpy()
     write_video(v, args.out, args.fps)
     print(f"{len(frames)} {'image' if len(frames) == 1 else 'keyframes'} -> {v.shape[0]} frames of "

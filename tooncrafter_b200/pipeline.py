@@ -34,6 +34,14 @@ whose c_concat is the image's latent repeated over the T frames.
 First stage: with the dual-reference AutoencoderKL_Dualref each segment is decoded twice (T = 16 and T = 14, then
 spliced, as above).  The plain AutoencoderKL of the DynamiCrafter / training configs decodes every frame on its own, so
 each segment is decoded once, without reference maps, and tc_video_u8 runs without a splice.
+
+Several GPUs (`ToonCrafterPipeline(model, group)`, one process per GPU): the S segments are split into contiguous
+blocks by distributed.shard_clips, one block per rank, or one per GPU pair with `latency` (the pair samples its block
+with DDIMSampler.latency_group, one guidance branch per GPU, and pair-rank 0 decodes).  Every rank still encodes all
+K keyframes and runs the two conditioning towers over the inputs of the single-process call, then takes its own
+rows: the batch sizes, and with them the kernels' tiling, are those of the single-process call.  By the RNG contract a
+segment is then the same computation whichever rank runs it; each block writes its contiguous range of the joined
+video, and the blocks are broadcast so that every rank returns the full video.
 """
 from __future__ import annotations
 
@@ -41,8 +49,9 @@ from typing import Optional, Sequence, Union
 
 import numpy as np
 import torch
+import torch.distributed as dist
 
-from . import ops, runtime
+from . import distributed, ops, runtime
 from .modules import VideoDecoder, clip_tokenize
 from .sampler import DDIMSampler, DDIMSamplerMultiCond
 
@@ -79,10 +88,31 @@ def default_segments_per_batch(size) -> int:
 
 
 class ToonCrafterPipeline:
-    """K keyframes -> one interpolated video, on a LatentVisualDiffusion of this library (see the module docstring)."""
+    """K keyframes -> one interpolated video, on a LatentVisualDiffusion of this library (see the module docstring).
 
-    def __init__(self, model):
+    group: None (one process; torch.distributed is not touched even when initialised), or a torch.distributed process
+    group whose ranks all construct the pipeline and make the same calls: the segments are sharded over its ranks and
+    every rank returns the full result of the single-process call.  latency: shard over GPU pairs (adjacent ranks of
+    `group`) instead, each pair sampling one block with one classifier-free-guidance branch per GPU; needs an even
+    group size, and refuses cfg_img and cfg_scale 1.0.  With `latency` every rank of the world must construct the
+    pipeline (the pair groups are created collectively)."""
+
+    def __init__(self, model, group=None, latency: bool = False):
         self.model = model
+        self.group = group
+        self.latency = latency
+        self._pair = None
+        if latency:
+            if group is None:
+                raise ValueError("latency mode needs a process group of GPU pairs")
+            self._pair, self._block, self._pair_rank = distributed.latency_pairs(group)
+            self._n_blocks = dist.get_world_size(group) // 2
+        elif group is not None:
+            self._block, self._n_blocks = dist.get_rank(group), dist.get_world_size(group)
+
+    def _owner(self, block: int) -> int:
+        """Global rank that holds block `block`'s result: the rank, or pair-rank 0 of the pair, that computes it."""
+        return dist.get_global_rank(self.group, 2 * block if self.latency else block)
 
     def _text(self, prompts, S: int):
         """(per-segment text embeddings [S, 77, D], the embedding of "" [1, 77, D]) from one text-tower pass."""
@@ -162,7 +192,43 @@ class ToonCrafterPipeline:
     def _generate(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
                   timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output) -> torch.Tensor:
         """S = len(first) segments; segment k runs from keyframe first[k] to keyframe last[k] (interp), or animates
-        keyframe first[k] (not interp)."""
+        keyframe first[k] (not interp).  With a group, this rank computes its block of segments and the blocks are
+        then broadcast."""
+        if self.latency:
+            if cfg_img is not None:
+                raise NotImplementedError("latency mode splits two guidance branches over a GPU pair; three-way "
+                                          "guidance (cfg_img) is not supported")
+            if cfg_scale == 1.0:
+                raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
+                                 "cfg_scale 1.0 has no unconditional branch")
+        T = self.model.temporal_length
+        S = len(first)
+        F = (T - 1) * S + (0 if loop else 1)
+        video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=self.model.device) if output == "uint8"
+                 else torch.empty(S, 3, T, size[0], size[1], dtype=torch.float32, device=self.model.device))
+        mine = list(range(S)) if self.group is None else distributed.shard_clips(S, self._block, self._n_blocks)
+        if mine:
+            self._render(frames, prompts, first, last, interp, steps, cfg_scale, eta, fs, guidance_rescale,
+                         timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video)
+        if self.group is None:
+            return video
+        blocks = []
+        for b in range(self._n_blocks):
+            seg = distributed.shard_clips(S, b, self._n_blocks)
+            if not seg:
+                continue
+            k0, k1 = seg[0], seg[-1]
+            if output == "float":
+                blocks.append((self._owner(b), k0, k1 + 1))
+            else:                                                   # the frames tc_video_u8 writes for the block
+                blocks.append((self._owner(b), (T - 1) * k0 + (1 if k0 else 0),
+                               (T - 1) * k1 + (T - 1 if (loop and k1 == S - 1) else T)))
+        distributed.broadcast_blocks(video, blocks, self.group)
+        return video
+
+    def _render(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
+                timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video) -> None:
+        """Sample and decode segments `mine` (of S = len(first)) into their places in `video`."""
         m = self.model
         dev = m.device
         T = m.temporal_length
@@ -170,6 +236,7 @@ class ToonCrafterPipeline:
         K, S = frames.shape[0], len(first)
 
         # conditioning: text over the distinct prompts + "", image over each segment's first keyframe + the zero image
+        # (over all S segments whatever `mine` is: the towers' batch size stays that of the single-process call)
         cond_emb, empty_emb = self._text(prompts, S)
         if m.uncond_type == "empty_seq":
             uc_emb = empty_emb.expand_as(cond_emb)
@@ -194,15 +261,14 @@ class ToonCrafterPipeline:
         else:
             c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
 
-        F = (T - 1) * S + (0 if loop else 1)
-        video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=dev) if output == "uint8" else
-                 torch.empty(S, 3, T, size[0], size[1], dtype=torch.float32, device=dev))
         sampler = DDIMSampler(m) if cfg_img is None else DDIMSamplerMultiCond(m)
-        dec = m.first_stage_model.decoder_engine()
+        sampler.latency_group = self._pair
+        decodes = not (self.latency and self._pair_rank)          # in a latency pair, pair-rank 0 decodes
+        dec = m.first_stage_model.decoder_engine() if decodes else None
         dual_ref = isinstance(m.first_stage_model.decoder, VideoDecoder)
         keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
-        for g0 in range(0, S, segments_per_batch):
-            seg = list(range(g0, min(g0 + segments_per_batch, S)))
+        for g0 in range(0, len(mine), segments_per_batch):
+            seg = mine[g0:g0 + segments_per_batch]
             b = len(seg)
             cc = [c_concat[seg]]
             cond = {"c_crossattn": [torch.cat([cond_emb[seg], img_emb[seg]], 1)], "c_concat": cc}
@@ -219,6 +285,8 @@ class ToonCrafterPipeline:
                                         fs=torch.tensor([fs] * b, dtype=torch.long, device=dev),
                                         timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale,
                                         noise_generators=gens, **extra)
+            if not decodes:
+                continue
             for i, k in enumerate(seg):
                 lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
                 if dual_ref:
@@ -245,4 +313,3 @@ class ToonCrafterPipeline:
                     ex(ops.video_u8, args, kw)
                 else:
                     ops.video_u8(*args, **kw)
-        return video

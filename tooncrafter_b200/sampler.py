@@ -301,7 +301,9 @@ class DDIMSampler(object):
         pred_x0 = torch.empty_like(x)
         if st.group is not None:
             from .distributed import sync_pair_state
-            sync_pair_state(x, st.group)                                   # same x_T and same noise stream on both ranks
+            # same x_T on both ranks, and the same noise: from pair-rank 0's global RNG stream, or from the per-row
+            # generators, which both ranks seed alike
+            sync_pair_state(x, st.group, rng_state=noise_generators is None)
         for i, (index, _) in enumerate(steps):
             noise = randn_rows(x.shape, st.dev, noise_generators)          # one draw per step, as ddim.py:273
             self._fused_step(st, i, x, noise, x_next, pred_x0)
