@@ -14,6 +14,10 @@ Reports per shape: microseconds per launch, TFLOP/s, launches per program and th
 library chose; per program the launch-weighted GEMM time and its TFLOP/s.  --sweep also times the --top shapes by
 FLOP share of a clip (50 UNet forwards + both decodes) under every legal block_n and k-slice cap.  Card name, power
 limit and SM clocks (query-only nvidia-smi) are recorded with the numbers.  Writes DIR/bench_gemm.json.
+
+Every shape whose epilogue reads a residual or a per-sample bias (bias2) is timed a second time without those operands,
+at the block_n and k-slices of the recorded call, so both runs use the same tiling.  The difference is what reading
+them costs; it is reported per shape ("operand_us") and summed over a clip ("epilogue_operands").
 """
 from __future__ import annotations
 
@@ -221,6 +225,17 @@ def main():
             row.update(rank=i, clip_flop_share=round(d["clip_flop"] / clip_flop, 4), us=round(us, 2),
                        tflops=round(d["flop"] / us / 1e6, 1), timed_launches=n,
                        config=dict(block_n=cfg["block_n"], ksplit=cfg["ksplit"], stages=cfg["stages"]))
+            if kw.get("res") is not None or kw.get("bias2") is not None:
+                # same tiling, no residual / bias2: block_n forced, k-slices capped at the recorded count
+                lib.tc_debug_set_gemm_mode(cfg["ksplit"] << 8)
+                kw0 = dict(kw, block_n=cfg["block_n"], res=None, bias2=None)
+                fn0 = lambda: ops.conv_gemm(*a, **kw0)
+                us0, _ = time_call(fn0, args.min_ms)
+                c0 = ops.last_gemm_config()
+                lib.tc_debug_set_gemm_mode(0)
+                assert (c0["block_n"], c0["ksplit"]) == (cfg["block_n"], cfg["ksplit"]), (c0, cfg)
+                row.update(us_without_operands=round(us0, 2), operand_us=round(us - us0, 2),
+                           config_without_operands=dict(block_n=c0["block_n"], ksplit=c0["ksplit"], stages=c0["stages"]))
             if args.sweep and i < args.top:
                 pts = []
                 for bn, cap in sweep_options(kw, k[1]):
@@ -237,6 +252,7 @@ def main():
                 row["chosen_over_best"] = round(us / best, 3)
             rows.append(row)
             print(json.dumps({x: row[x] for x in ("rank", "M", "N", "K", "taps", "us", "tflops", "config")}
+                             | {x: row[x] for x in ("operand_us", "config_without_operands") if x in row}
                              | ({"chosen_over_best": row["chosen_over_best"]} if "sweep" in row else {})), flush=True)
             del a, kw
             torch.cuda.empty_cache()
@@ -250,17 +266,25 @@ def main():
         programs[p] = dict(launches=len(progs[p]), gemm_ms=round(ms, 3), tflop=round(fl / 1e12, 3),
                            tflops=round(fl / ms / 1e9, 1) if ms else None)
     clip_ms = sum(programs[p]["gemm_ms"] * RUNS_PER_CLIP[p] for p in programs)
+    clip_launches = lambda r: sum(n * RUNS_PER_CLIP[p] for p, n in r["launches"].items())
+    abl = [r for r in rows if "operand_us" in r]
+    op_ms = sum(r["operand_us"] * clip_launches(r) for r in abl) / 1e3
+    epi_ops = dict(shapes=len(abl), clip_launches=sum(clip_launches(r) for r in abl),
+                   clip_ms_with=round(sum(r["us"] * clip_launches(r) for r in abl) / 1e3, 1),
+                   clip_ms_without=round(sum(r["us_without_operands"] * clip_launches(r) for r in abl) / 1e3, 1),
+                   clip_operand_ms=round(op_ms, 1), share_of_clip_gemm=round(op_ms / clip_ms, 4) if clip_ms else None)
     out = dict(metric="tc_conv_gemm per-shape time at the shapes of one clip (synthetic fp16 operands, CUDA graph of "
                       "back-to-back launches, CUDA events)",
                gpu=info, clocks_during_run=clk, min_ms_per_shape=args.min_ms, plan_s=round(plan_s, 1),
                programs=programs, runs_per_clip=RUNS_PER_CLIP,
                clip=dict(gemm_ms=round(clip_ms, 1), tflop=round(clip_flop / 1e12, 1),
                          tflops=round(clip_flop / clip_ms / 1e9, 1)),
-               shapes=rows)
+               epilogue_operands=epi_ops, shapes=rows)
     od = Path(args.out)
     od.mkdir(parents=True, exist_ok=True)
     (od / "bench_gemm.json").write_text(json.dumps(out, indent=1))
-    print(json.dumps(dict(gpu=info, clocks_during_run=clk, programs=programs, clip=out["clip"])), flush=True)
+    print(json.dumps(dict(gpu=info, clocks_during_run=clk, programs=programs, clip=out["clip"],
+                           epilogue_operands=epi_ops)), flush=True)
     return 0
 
 

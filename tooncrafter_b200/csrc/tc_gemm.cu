@@ -6,7 +6,12 @@
 //   warpgroup 0    TMA producer  : one elected thread; per k-block one 4-D box of the channels-last activation (im2col
 //                                  by coordinate offset; out-of-bounds rows/cols are zero-filled by TMA == padding) and
 //                                  one 2-D box of the [Cout][taps*C] weight matrix, both 128B-swizzled, into a ring of
-//                                  `stages` shared-memory slots guarded by full / empty mbarriers.
+//                                  `stages` shared-memory slots guarded by full / empty mbarriers.  Before the first
+//                                  k-block it issues the tile's residual (32-column boxes, 64B-swizzled) into a region
+//                                  of its own, on an mbarrier of its own, so the residual lands during the k-loop.
+//                  warps 1-3     : during the k-loop, per-row LayerNorm statistics (partial slots summed) and the bias2
+//                                  rows the tile spans, into shared memory (named barrier 2).  The epilogue therefore
+//                                  reads no global memory, and its stores do not wait behind its loads.
 //   warpgroups 1-2 wgmma         : each owns 64 of the tile's 128 rows; one m64nNk16 instruction per k16 step with
 //                                  N = BNp (BN rounded up to 32), so A is read from shared memory once per step for all
 //                                  columns; fp32 accumulators in registers, one k-block in flight behind the one being
@@ -34,9 +39,19 @@ constexpr int kAStageBytes = kBlockM * kBlockK * 2;  // 16 KiB
 constexpr int kThreads = 384;                        // warpgroup 0 TMA, warpgroups 1-2 MMA + epilogue
 constexpr int kEpiThreads = 256;
 
+constexpr int kResBoxCols = 32;                      // residual box: 32 halfs = one 64-byte swizzle row
+constexpr int kResBoxBytes = kBlockM * kResBoxCols * 2;   // 8 KiB region per residual box
+
 struct alignas(64) GemmKParams {
     CUtensorMap tmA;
     CUtensorMap tmB;
+    CUtensorMap tmR;                // residual [oN][oH][oW][n_cols] (row stride ldr), boxes of 32 columns
+    int res_boxes;                  // residual boxes per tile (ceil(BN / 32)), 0 without a residual
+    uint32_t res_bytes;             // residual bytes delivered per tile
+    uint32_t res_smem;              // shared-memory region of the residual boxes (res_boxes x 8 KiB)
+    uint32_t b2_smem;               // shared-memory region of the staged bias2 rows (slots x BN halfs)
+    int b2_per_row;                 // 1: one bias2 slot per tile row (a tile spans more bias2 rows than it has rows);
+                                    // 0: one slot per bias2 row the tile spans, from its first output row's
     int taps;
     int tap_dx[TC_MAX_TAPS], tap_dy[TC_MAX_TAPS], tap_dn[TC_MAX_TAPS];
     int kc_per_tap;
@@ -59,8 +74,6 @@ struct alignas(64) GemmKParams {
     const __half* bias2;
     long long bias2_ld;
     int bias2_rows_per;
-    const __half* res;
-    long long ldr;
     float acc_scale;
     int geglu;
     const float2* ln_stats;  // per output row {mean, rstd} (ln_nslots == 0) or [M][ln_nslots] partial {sum, sumsq}
@@ -74,6 +87,22 @@ struct alignas(64) GemmKParams {
 __device__ __forceinline__ uint32_t pack_h2(float x, float y) {
     __half2 h = __floats2half2_rn(x, y);
     return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// output row m of tile row `row` (rows in the box's (TW, TH, TN) order, x fastest); false past the output extent
+__device__ __forceinline__ bool tile_row(const GemmKParams& p, int tx, int ty, int tn, int row, long long& m) {
+    const int rx = row % p.TW;
+    const int ry = (row / p.TW) % p.TH;
+    const int rn = row / (p.TW * p.TH);
+    const int x = tx * p.TW + rx, y = ty * p.TH + ry, n = tn * p.TN + rn;
+    m = ((long long)n * p.oH + y) * p.oW + x;
+    return (rn < p.TN) && (x < p.oW) && (y < p.oH) && (n < p.oN);
+}
+
+// bias2 row of the tile's first output row
+__device__ __forceinline__ long long tile_bias2_first(const GemmKParams& p, int tx, int ty, int tn) {
+    const long long m0 = ((long long)tn * p.TN * p.oH + ty * p.TH) * p.oW + tx * p.TW;
+    return m0 / p.bias2_rows_per;
 }
 
 // kNJ = BNp / 32 (BNp = BN rounded up to 32): the wgmma is m64n(32 kNJ)k16
@@ -90,21 +119,27 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     uint8_t* sA = smem;
     uint8_t* sB = smem + (size_t)S * kAStageBytes;
     float* stg = reinterpret_cast<float*>(smem);   // [128][kLds] fp32 accumulators, after the ring has drained
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.ring_bytes);
+    uint8_t* s_res = smem + p.ring_bytes;          // residual boxes: [res_boxes][128 rows][64 B], 64B-swizzled
+    __half* s_b2 = reinterpret_cast<__half*>(s_res + p.res_smem);   // [bias2_rows_max][BN]
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_res + p.res_smem + p.b2_smem);
     uint64_t* empty_bar = full_bar + S;
-    float* s_bias = reinterpret_cast<float*>(empty_bar + S);   // [256]
+    uint64_t* res_bar = empty_bar + S;
+    float* s_bias = reinterpret_cast<float*>(res_bar + 1);     // [256]
     float* s_u = s_bias + 256;                                 // [256]
     float2* s_rs = reinterpret_cast<float2*>(s_u + 256);       // [128] row statistics of column group 1
-    int* s_flag = reinterpret_cast<int*>(s_rs + 128);
+    float2* s_ln = s_rs + 128;                                 // [128] per-row LayerNorm {mean, rstd}
+    int* s_flag = reinterpret_cast<int*>(s_ln + 128);
 
     const int tid = threadIdx.x;
     if (tid == 0) {
         tc::tma_prefetch_desc(&p.tmA);
         tc::tma_prefetch_desc(&p.tmB);
+        if (p.res_boxes) tc::tma_prefetch_desc(&p.tmR);
         for (int s = 0; s < S; ++s) {
             tc::mbar_init(&full_bar[s], 1);
             tc::mbar_init(&empty_bar[s], 8);   // one arrival per consumer warp
         }
+        tc::mbar_init(res_bar, 1);
         tc::fence_mbar_init();
     }
     __syncthreads();
@@ -123,10 +158,79 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     const int kb_begin = ks * p.kb_per;
     const int kb_end = min(kb_begin + p.kb_per, main_kblocks);
 
-    if (tid < 128) {
+    if (tid >= 32 && tid < 128) {
+        // ------------------------------------------------------------------ warps 1-3: epilogue operands, during the k-loop
+        // per-row LayerNorm statistics (partial slots summed in slot order, as a fixed order keeps results deterministic)
+        // and the bias2 rows of the tile; the MMA warpgroups wait for them (named barrier 2) only after their k-loop
+        const int pt = tid - 32;
+        if (p.ln_stats) {
+            for (int row = pt; row < kBlockM; row += 96) {
+                long long m;
+                float mean = 0.f, rstd = 1.f;
+                if (tile_row(p, tx, ty, tn, row, m)) {
+                    if (p.ln_nslots > 0) {
+                        float s1 = 0.f, s2 = 0.f;
+                        const float2* ps = p.ln_stats + m * p.ln_nslots;
+                        for (int i = 0; i < p.ln_nslots; ++i) {
+                            const float2 st = __ldg(ps + i);
+                            s1 += st.x;
+                            s2 += st.y;
+                        }
+                        mean = s1 * p.ln_inv_c;
+                        rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
+                    } else {
+                        const float2 st = __ldg(p.ln_stats + m);
+                        mean = st.x;
+                        rstd = st.y;
+                    }
+                }
+                s_ln[row] = make_float2(mean, rstd);
+            }
+        }
+        if (p.bias2) {
+            // slots: bias2 rows [first, last] of the tile's first and last output rows (a tile may straddle sample
+            // boundaries), or the bias2 row of each tile row (b2_per_row); columns past n_cols are zero (they feed no
+            // stored output)
+            long long m_last;
+            const int xl = min(p.TW, p.oW - tx * p.TW) - 1, yl = min(p.TH, p.oH - ty * p.TH) - 1;
+            const int nl = min(p.TN, p.oN - tn * p.TN) - 1;
+            tile_row(p, tx, ty, tn, (nl * p.TH + yl) * p.TW + xl, m_last);
+            const long long first = tile_bias2_first(p, tx, ty, tn);
+            const int slots = p.b2_per_row ? kBlockM : (int)(m_last / p.bias2_rows_per - first) + 1;
+            const int chunks = BN / 8;
+            for (int i = pt; i < slots * chunks; i += 96) {
+                const int r = i / chunks, c = 8 * (i - r * chunks);
+                const int col = nt * BN + c;
+                long long b2r = first + r;
+                if (p.b2_per_row) {
+                    long long m;
+                    if (!tile_row(p, tx, ty, tn, r, m)) continue;
+                    b2r = m / p.bias2_rows_per;
+                }
+                const __half* src = p.bias2 + b2r * p.bias2_ld + col;
+                __half* dst = s_b2 + r * BN + c;
+                if (col + 8 <= p.n_cols) {
+                    *reinterpret_cast<uint4*>(dst) = __ldg(reinterpret_cast<const uint4*>(src));
+                } else {
+                    for (int j = 0; j < 8; ++j) dst[j] = col + j < p.n_cols ? src[j] : __float2half_rn(0.f);
+                }
+            }
+        }
+        asm volatile("bar.arrive 2, 352;" ::: "memory");
+        return;
+    }
+    if (tid < 32) {
         // ------------------------------------------------------------------ TMA producer
-        if (tid < 32 && tc::elect_one()) {
+        if (tc::elect_one()) {
             const int x0 = tx * p.TW, y0 = ty * p.TH, n0 = tn * p.TN;
+            if (p.res_boxes) {
+                // the residual tile lands during the k-loop, on an mbarrier of its own.  Under split-K every slice loads
+                // it: which slice runs the epilogue is known only from its ticket, after its k-loop, and one more
+                // 128 x BN fp16 read is small next to a slice's operand traffic (>= 8 k-blocks of A and B)
+                tc::mbar_arrive_expect_tx(res_bar, p.res_bytes);
+                for (int b = 0; b < p.res_boxes; ++b)
+                    tc::tma_load_4d(s_res + b * kResBoxBytes, &p.tmR, res_bar, nt * BN + b * kResBoxCols, x0, y0, n0);
+            }
             int stage = 0;
             uint32_t phase = 0;
             int tap = kb_begin / p.kc_per_tap;
@@ -182,8 +286,11 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
         }
         tc::wgmma_wait<0>();
     }
-    // every MMA of both warpgroups has retired: the operand ring becomes the accumulator staging tile
-    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // every MMA of both warpgroups has retired (the operand ring becomes the accumulator staging tile), and warps 1-3
+    // have stored the LayerNorm statistics and bias2 rows
+    asm volatile("bar.sync 2, 352;" ::: "memory");
+    // every k-slice waits, so that no CTA exits with its residual load in flight
+    if (p.res_boxes) tc::mbar_wait(res_bar, 0);
     {
         const int r0 = wg * 64 + warp * 16 + (lane >> 2);
 #pragma unroll
@@ -232,12 +339,8 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     // ---------------------------------------------------------------------- epilogue: one row per thread, 2 column groups
     const int row = et & 127;
     const int cg = et >> 7;
-    const int rx = row % p.TW;
-    const int ry = (row / p.TW) % p.TH;
-    const int rn = row / (p.TW * p.TH);
-    const int x = tx * p.TW + rx, y = ty * p.TH + ry, n = tn * p.TN + rn;
-    const bool row_ok = (rn < p.TN) && (x < p.oW) && (y < p.oH) && (n < p.oN);
-    const long long m = ((long long)n * p.oH + y) * p.oW + x;
+    long long m;
+    const bool row_ok = tile_row(p, tx, ty, tn, row, m);
     const bool geglu = p.geglu != 0;
     const int width = geglu ? (BN >> 1) : BN;                   // output columns per tile
     const int split = ((width / 16 + 1) / 2) * 16;              // group 0: [0, split), group 1: [split, width)
@@ -247,27 +350,18 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     const int col0 = nt * width;                                // first output column of the tile
 
     float mean = 0.f, rstd = 1.f;
-    if (p.ln_stats && row_ok) {
-        if (p.ln_nslots > 0) {
-            // partial {sum, sumsq} slots written by the producer GEMM's epilogue (fixed order: deterministic)
-            float s1 = 0.f, s2 = 0.f;
-            const float2* ps = p.ln_stats + m * p.ln_nslots;
-            for (int i = 0; i < p.ln_nslots; ++i) {
-                const float2 st = __ldg(ps + i);
-                s1 += st.x;
-                s2 += st.y;
-            }
-            mean = s1 * p.ln_inv_c;
-            rstd = rsqrtf(fmaxf(s2 * p.ln_inv_c - mean * mean, 0.f) + p.ln_eps);
-        } else {
-            const float2 st = __ldg(p.ln_stats + m);
-            mean = st.x;
-            rstd = st.y;
-        }
+    if (p.ln_stats) {
+        const float2 st = s_ln[row];
+        mean = st.x;
+        rstd = st.y;
     }
     const float* srow = stg + row * kLds;
-    const __half* b2row = (p.bias2 && row_ok) ? p.bias2 + (m / p.bias2_rows_per) * p.bias2_ld + (long long)nt * BN : nullptr;
-    const __half* rrow = (p.res && row_ok) ? p.res + m * p.ldr + (long long)nt * BN : nullptr;
+    const __half* b2row = (p.bias2 && row_ok)
+                              ? s_b2 + (p.b2_per_row ? row : m / p.bias2_rows_per - tile_bias2_first(p, tx, ty, tn)) * BN
+                              : nullptr;
+    // residual: 16-byte chunk q of a 64-byte box row sits at chunk q ^ ((row >> 1) & 3) (CU_TENSOR_MAP_SWIZZLE_64B)
+    const uint8_t* rrow = s_res + row * (kResBoxCols * 2);
+    const int rswz = (row >> 1) & 3;
     __half* orow = p.out + m * p.ldc + col0;
     float rs_sum = 0.f, rs_sq = 0.f;
     if (row_ok) {
@@ -279,35 +373,28 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
 #pragma unroll
                 for (int i = 0; i < 8; ++i) v[i] = rstd * (srow[c + i] - mean * s_u[c + i]) + s_bias[c + i];
                 if (b2row) {
-                    if (nvalid == 8) {
-                        const uint4 u = __ldg(reinterpret_cast<const uint4*>(b2row + c));
-                        const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+                    const uint4 u = *reinterpret_cast<const uint4*>(b2row + c);
+                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float2 f = __half22float2(h2[i]);
-                            v[2 * i] += f.x;
-                            v[2 * i + 1] += f.y;
-                        }
-                    } else {
-                        for (int i = 0; i < nvalid; ++i) v[i] += __half2float(b2row[c + i]);
+                    for (int i = 0; i < 4; ++i) {
+                        const float2 f = __half22float2(h2[i]);
+                        v[2 * i] += f.x;
+                        v[2 * i + 1] += f.y;
                     }
                 }
                 if (p.acc_scale != 1.0f) {
 #pragma unroll
                     for (int i = 0; i < 8; ++i) v[i] *= p.acc_scale;
                 }
-                if (rrow) {
-                    if (nvalid == 8) {
-                        const uint4 u = *reinterpret_cast<const uint4*>(rrow + c);
-                        const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+                if (p.res_boxes) {
+                    const uint4 u = *reinterpret_cast<const uint4*>(
+                        rrow + (c / kResBoxCols) * kResBoxBytes + ((((c >> 3) & 3) ^ rswz) << 4));
+                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const float2 f = __half22float2(h2[i]);
-                            v[2 * i] += f.x;
-                            v[2 * i + 1] += f.y;
-                        }
-                    } else {
-                        for (int i = 0; i < nvalid; ++i) v[i] += __half2float(rrow[c + i]);
+                    for (int i = 0; i < 4; ++i) {
+                        const float2 f = __half22float2(h2[i]);
+                        v[2 * i] += f.x;
+                        v[2 * i + 1] += f.y;
                     }
                 }
             } else {
@@ -462,7 +549,7 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     TC_CHECK_ARG(!d->res || (d->ldr % 8 == 0 && (reinterpret_cast<uintptr_t>(d->res) & 15) == 0),
                  "tc_conv_gemm: residual must be 16-byte aligned");
     TC_CHECK_ARG(!d->res || d->ldr >= d->n_cols, "tc_conv_gemm: ldr must be >= n_cols");
-    // the epilogue reads bias2 8 halfs (16 bytes) at a time
+    // bias2 rows are staged into shared memory 8 halfs (16 bytes) at a time
     TC_CHECK_ARG(!d->bias2 || (d->bias2_ld % 8 == 0 && (reinterpret_cast<uintptr_t>(d->bias2) & 15) == 0),
                  "tc_conv_gemm: bias2 must be 16-byte aligned with bias2_ld % 8 == 0");
     TC_CHECK_ARG(d->n_cols <= d->b_rows, "tc_conv_gemm: n_cols must be <= b_rows");
@@ -548,8 +635,6 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     p.bias2 = reinterpret_cast<const __half*>(d->bias2);
     p.bias2_ld = d->bias2_ld;
     p.bias2_rows_per = d->bias2_rows_per > 0 ? d->bias2_rows_per : 1;
-    p.res = reinterpret_cast<const __half*>(d->res);
-    p.ldr = d->ldr;
     p.acc_scale = d->acc_scale;
     p.geglu = geglu ? 1 : 0;
     p.ln_stats = reinterpret_cast<const float2*>(d->ln_stats);
@@ -580,20 +665,42 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
         if (!m) return TC_ERR_CUDA;
         p.tmB = *m;
     }
+    if (d->res) {
+        // the output tile's (TW, TH, TN) box over the residual, cut into 32-column boxes (64-byte swizzle): 32 rather
+        // than 64 columns so that a 160-wide tile takes 40 KiB rather than 48 KiB, which keeps its ring at 5 stages
+        uint64_t dims[4] = {(uint64_t)d->n_cols, (uint64_t)d->oW, (uint64_t)d->oH, (uint64_t)d->oN};
+        uint64_t strides[3] = {(uint64_t)d->ldr * 2, (uint64_t)d->ldr * d->oW * 2, (uint64_t)d->ldr * d->oW * d->oH * 2};
+        uint32_t box[4] = {(uint32_t)kResBoxCols, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TN};
+        const CUtensorMap* m = get_tensor_map(d->res, 4, dims, strides, box, 64);
+        if (!m) return TC_ERR_CUDA;
+        p.tmR = *m;
+        p.res_boxes = (BN + kResBoxCols - 1) / kResBoxCols;
+        p.res_bytes = (uint32_t)(p.res_boxes * p.TW * p.TH * p.TN * kResBoxCols * 2);
+        p.res_smem = (uint32_t)(p.res_boxes * kResBoxBytes);
+    }
+    if (d->bias2) {
+        // bias2 rows one tile can span: its output rows lie within `extent` rows of its first one.  A conv box with
+        // TW < oW or TH < oH spans more than 128 consecutive output rows; past 128 bias2 rows, stage one per tile row
+        const long long extent = ((long long)(p.TN - 1) * p.oH + (p.TH - 1)) * p.oW + (p.TW - 1);
+        const long long span = (extent + p.bias2_rows_per - 1) / p.bias2_rows_per + 1;
+        p.b2_per_row = span > kBlockM ? 1 : 0;
+        p.b2_smem = (uint32_t)((p.b2_per_row ? kBlockM : span) * BN * 2);
+    }
 
-    // shared memory: operand ring (at least as large as the fp32 staging tile it becomes), barriers, per-column vectors,
-    // row-statistics hand-over, alignment slack
+    // shared memory: operand ring (at least as large as the fp32 staging tile it becomes), residual boxes, bias2 rows,
+    // barriers, per-column vectors, per-row statistics, alignment slack
     const int stage_bytes = kAStageBytes + (int)p.b_bytes;
     const int staging_bytes = kBlockM * (BNp + 4) * 4;
-    const int kFixedSmem = 1024 + 8 * 2 * 8 + 2048 + 1024 + 64;
-    const int smem_budget = 227 * 1024 - kFixedSmem;
+    const int kFixedSmem = 1024 + 8 * (2 * 8 + 1) + 2048 + 1024 + 1024 + 64;
+    const int operand_smem = (int)(p.res_smem + p.b2_smem);
+    const int smem_budget = 227 * 1024 - kFixedSmem - operand_smem;
     int stages = smem_budget / stage_bytes;
     if (stages > 8) stages = 8;
     if (stages < 2) return fail(TC_ERR_INVALID, "tc_conv_gemm: not enough shared memory for 2 stages");
     p.stages = stages;
     const int ring = stages * stage_bytes > staging_bytes ? stages * stage_bytes : staging_bytes;
     p.ring_bytes = (uint32_t)ring;
-    const size_t smem_bytes = (size_t)ring + kFixedSmem;
+    const size_t smem_bytes = (size_t)ring + operand_smem + kFixedSmem;
     TC_CHECK_ARG(smem_bytes <= 227 * 1024, "tc_conv_gemm: tile does not fit in shared memory");
 
     static bool attr_set = false;
