@@ -164,7 +164,7 @@ typedef struct {
 int tc_attention(const TcAttention* desc, void* stream);
 
 /* Temporal self-attention over the frame axis (attention.py:365-412 'only_self_att', einsum path :103-120):
- * tokens x[b][t][p][heads*64]; for each (b, p, head) softmax(q k^T * scale) v over t in [0,T), T <= 32.
+ * tokens x[b][t][p][heads*64]; for each (b, p, head) softmax(q k^T * scale) v over t in [0,T), T <= 64.
  * Refused: q, k, v or out not 16-byte aligned, ld or ldo not a multiple of 8 or below heads*64. */
 int tc_temporal_attention(const void* q, const void* k, const void* v, long long ld, void* out, long long ldo,
                           int B, int T, int P, int heads, float scale, void* stream);

@@ -17,6 +17,12 @@ events, 10 replays after a warm-up):
 
     python scripts/bench_pipeline.py --animate --first-stage plain --size 576 1024
 
+--video-length T [T ...] measures a K = 2 interpolate() with T frames per segment at --size with --first-stage, for
+each T in turn: seconds per video and frames/s (warm-up at DDIM-2, then `--reps` timed calls) and the peak device
+memory of a timed call.  Each T starts from freshly built engines, so its peak holds its own plans only:
+
+    python scripts/bench_pipeline.py --video-length 8 16 24 32 64
+
 --gpus N measures ToonCrafterPipeline sharded over N GPUs, one process per GPU under torchrun (--gpus 1: the same
 workload on one GPU, without torchrun): a K = 5 interpolate() at --size, or with --animate one animate() call, with
 --latency-mode one clip per GPU pair.  Warm-up at DDIM-2, then `--reps` timed calls, each between a barrier and a
@@ -152,6 +158,38 @@ def bench_animate(args, model, info, build_s, decode16):
     return 0
 
 
+def bench_video_length(args, model, info, build_s):
+    """K = 2 interpolate at each T of args.video_length (see the module docstring)."""
+    from tooncrafter_b200.pipeline import ToonCrafterPipeline
+    size = tuple(args.size)
+    pipe = ToonCrafterPipeline(model)
+    kf = (torch.rand(2, size[0], size[1], 3, generator=torch.Generator().manual_seed(0)) * 255).to(torch.uint8)
+    rows = []
+    for T in args.video_length:
+        model.model.diffusion_model._engine = None                  # this T's plans only in the peak
+        model.first_stage_model._dec_engine = None
+        torch.cuda.empty_cache()
+        run = lambda st: pipe.interpolate(kf, steps=st, seed=123, size=size, video_length=T)   # noqa: E731
+        run(2)
+        times, peak = [], 0
+        for _ in range(args.reps):
+            dt, pk = _timed(lambda: run(args.ddim_steps))
+            times.append(dt)
+            peak = max(peak, pk)
+        best = min(times)
+        row = dict(video_length=T, frames=T, sec_per_video=best, frames_per_s=T / best,
+                   all_s=[round(x, 3) for x in times], peak_gib=peak / 2 ** 30)
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    out = dict(metric="K = 2 interpolation by frames per segment: seconds per video (%dx%d, DDIM-%d, CFG 7.5, eta 1, "
+               "synthetic weights, %s first stage)" % (size[0], size[1], args.ddim_steps, args.first_stage), gpu=info,
+               reps=args.reps, model_build_s=build_s, configs=rows,
+               note="sec_per_video = best of the timed reps, host clock around work ending in a device synchronise; "
+                    "peak_gib = torch.cuda.max_memory_allocated over a timed call")
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def bench_sharded(args, model, info, build_s, group):
     """--gpus N: K = 5 interpolate (or animate) sharded over `group` (None: one GPU); see the module docstring."""
     import torch.distributed as dist
@@ -201,7 +239,16 @@ def main():
     ap.add_argument("--gpus", type=int, default=None,
                     help="measure the pipeline sharded over N GPUs, under torchrun when N > 1 (docstring)")
     ap.add_argument("--latency-mode", action="store_true", help="with --gpus: one clip per GPU pair")
+    ap.add_argument("--video-length", type=int, nargs="+", default=None, metavar="T",
+                    help="measure K = 2 interpolation at each of these frames-per-segment counts (docstring)")
     args = ap.parse_args()
+    if args.video_length is not None:
+        from tooncrafter_b200.pipeline import check_video_length
+        try:
+            for T in args.video_length:
+                check_video_length(T)
+        except ValueError as e:
+            ap.error(str(e))
     from tooncrafter_b200 import synthetic
     from tooncrafter_b200.pipeline import ToonCrafterPipeline
     if not torch.cuda.is_available():
@@ -235,6 +282,8 @@ def main():
                 torch.distributed.destroy_process_group()
     if args.animate:
         return bench_animate(args, model, info, build_s, decode16)
+    if args.video_length is not None:
+        return bench_video_length(args, model, info, build_s)
     pipe = ToonCrafterPipeline(model)
     g = torch.Generator().manual_seed(0)
     results = []

@@ -6,7 +6,8 @@
 //                         text tower).
 //  tc_attention_wide      the same kernel for one head of up to 512 channels (VAE mid-block attention): scores stay
 //                         on chip; each CTA produces 256, 128 or 64 of the value channels (the widest that divides D).
-//  tc_temporal_attention  16-frame temporal self-attention, one (pixel, head) per warp, mma.sync 16x8x16 (HBM-bound).
+//  tc_temporal_attention  temporal self-attention over T <= 64 frames, one (pixel, head) per warp, mma.sync 16x8x16
+//                         (HBM-bound): one kernel for T <= 16, one for 16 < T <= 64.
 //  tc_softmax_rows        row softmax over a stored score matrix.
 //
 // Reference sites: lvdm/modules/attention.py:81-209,365-412; lvdm/models/autoencoder_dualref.py:172-200,270-341.
@@ -271,112 +272,6 @@ __global__ void __launch_bounds__(kFaThreads) flash_attn_kernel(const FaParams p
     }
 }
 
-// ===================================================================================== temporal attention
-// x[b][t][p][heads*64]; one (b, p, head) item per group of kGroup lanes (lane i of the group = query frame i).
-template <int kGroup>
-__global__ void temporal_attn_kernel(const __half* __restrict__ q, const __half* __restrict__ k,
-                                     const __half* __restrict__ v, long long ld, __half* __restrict__ out,
-                                     long long ldo, int B, int T, int P, int heads, float scale_log2) {
-    tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
-    constexpr int kItemsPerWarp = 32 / kGroup;
-    constexpr int kWarps = 4;
-    __shared__ __align__(16) __half sK[kWarps * kItemsPerWarp][kGroup][64];
-    __shared__ __align__(16) __half sV[kWarps * kItemsPerWarp][kGroup][64];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int sub = lane / kGroup, t = lane % kGroup;
-    const long long total = (long long)B * P * heads;
-    const long long item = ((long long)blockIdx.x * kWarps + warp) * kItemsPerWarp + sub;
-    const bool item_ok = item < total;
-    const int slot = warp * kItemsPerWarp + sub;
-
-    long long b = 0, pix = 0;
-    int h = 0;
-    if (item_ok) {
-        h = (int)(item % heads);
-        const long long r = item / heads;
-        pix = r % P;
-        b = r / P;
-    }
-    const bool row_ok = item_ok && t < T;
-    const long long tok = ((b * T + t) * P + pix);
-    float qf[64];
-    if (row_ok) {
-        const uint4* qp = reinterpret_cast<const uint4*>(q + tok * ld + h * 64);
-        const uint4* kp = reinterpret_cast<const uint4*>(k + tok * ld + h * 64);
-        const uint4* vp = reinterpret_cast<const uint4*>(v + tok * ld + h * 64);
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-            const uint4 u = qp[c];
-            const __half2* hh = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const float2 f = __half22float2(hh[i]);
-                qf[c * 8 + 2 * i] = f.x;
-                qf[c * 8 + 2 * i + 1] = f.y;
-            }
-            reinterpret_cast<uint4*>(&sK[slot][t][0])[c] = kp[c];
-            reinterpret_cast<uint4*>(&sV[slot][t][0])[c] = vp[c];
-        }
-    }
-    __syncwarp();
-    if (!row_ok) return;
-
-    float s[kGroup];
-    float m = -INFINITY;
-#pragma unroll
-    for (int j = 0; j < kGroup; ++j) {
-        if (j < T) {
-            float acc = 0.f;
-            const __half2* kr = reinterpret_cast<const __half2*>(&sK[slot][j][0]);
-#pragma unroll
-            for (int d = 0; d < 32; ++d) {
-                const float2 f = __half22float2(kr[d]);
-                acc += qf[2 * d] * f.x + qf[2 * d + 1] * f.y;
-            }
-            s[j] = acc * scale_log2;
-            m = fmaxf(m, s[j]);
-        }
-    }
-    float l = 0.f;
-#pragma unroll
-    for (int j = 0; j < kGroup; ++j) {
-        if (j < T) {
-            s[j] = exp2f(s[j] - m);
-            l += s[j];
-        }
-    }
-    const float inv = 1.0f / l;
-    float o[64];
-#pragma unroll
-    for (int d = 0; d < 64; ++d) o[d] = 0.f;
-#pragma unroll
-    for (int j = 0; j < kGroup; ++j) {
-        if (j < T) {
-            const float pj = s[j] * inv;
-            const __half2* vr = reinterpret_cast<const __half2*>(&sV[slot][j][0]);
-#pragma unroll
-            for (int d = 0; d < 32; ++d) {
-                const float2 f = __half22float2(vr[d]);
-                o[2 * d] += pj * f.x;
-                o[2 * d + 1] += pj * f.y;
-            }
-        }
-    }
-    __half* dst = out + tok * ldo + h * 64;
-#pragma unroll
-    for (int c = 0; c < 8; ++c) {
-        __half2 hh[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) hh[i] = __floats2half2_rn(o[c * 8 + 2 * i], o[c * 8 + 2 * i + 1]);
-        uint4 u;
-        u.x = *reinterpret_cast<uint32_t*>(&hh[0]);
-        u.y = *reinterpret_cast<uint32_t*>(&hh[1]);
-        u.z = *reinterpret_cast<uint32_t*>(&hh[2]);
-        u.w = *reinterpret_cast<uint32_t*>(&hh[3]);
-        reinterpret_cast<uint4*>(dst)[c] = u;
-    }
-}
-
 // ===================================================================================== temporal attention, T <= 16
 // One warp per (batch, pixel, head): the whole problem is a 16 x 16 x 64 attention, far below a 64-row wgmma tile,
 // and the kernel is HBM-bound (reads q, k, v once, writes o once).  S = Q K^T and O = P V use warp-level
@@ -503,6 +398,160 @@ __global__ void __launch_bounds__(128) temporal_attn_mma_kernel(const __half* __
             }
         }
         __syncwarp();   // smem V tile is reused by the next item
+    }
+}
+
+// ===================================================================================== temporal attention, 16 < T <= 64
+// One warp per (batch, pixel, head), kTiles = ceil(T / 16) tiles of 16 frames.  K and V (T x 64 fp16 each, up to
+// 8 KiB) are staged by cp.async into this warp's swizzled smem tiles, zero-filled past frame T; K feeds the B operand
+// of S = Q K^T by ldmatrix, V the B operand of O = P V by ldmatrix.trans.  Each 16-row query tile computes its scores
+// against all T keys at once, so the softmax is exact (no running maximum), in fp32 on the accumulator fragments.
+// Dynamic smem: 4 warps x (K + V) x kTiles * 2 KiB, room for 6, 4 or 3 CTAs per SM at kTiles = 2, 3, 4; the register
+// bound asks for 5 (6 would spill), 4 and 3.
+template <int kTiles>
+__global__ void __launch_bounds__(128, kTiles == 2 ? 5 : 12 / kTiles) temporal_attn_mma64_kernel(const __half* __restrict__ q,
+                                                                  const __half* __restrict__ k,
+                                                                  const __half* __restrict__ v, long long ld,
+                                                                  __half* __restrict__ out, long long ldo, int B, int T,
+                                                                  int P, int heads, float scale_log2) {
+    tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
+    constexpr int kRows = 16 * kTiles;
+    constexpr int kTileBytes = kRows * 128;
+    extern __shared__ __align__(128) uint8_t tsmem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int g = lane >> 2, t4 = lane & 3;
+    const uint32_t sK = tc::smem_u32(tsmem) + (uint32_t)(warp * 2 * kTileBytes);
+    const uint32_t sV = sK + (uint32_t)kTileBytes;
+    const long long total = (long long)B * P * heads;
+    const long long frame_stride = (long long)P * ld;       // elements between consecutive frames of one pixel
+    for (long long item = (long long)blockIdx.x * 4 + warp; item < total; item += (long long)gridDim.x * 4) {
+        const int h = (int)(item % heads);
+        const long long r = item / heads;
+        const long long pix = r % P, b = r / P;
+        const long long base = ((b * T) * P + pix) * ld + h * 64;   // frame 0 of this (b, pix, head)
+        // ---- K, then V -> smem (two cp.async groups: S runs while V lands); frames >= T are zeros
+#pragma unroll
+        for (int i = 0; i < kRows * 8 / 32; ++i) {
+            const int chunk = lane + 32 * i, row = chunk >> 3, c16 = chunk & 7;
+            const bool ok = row < T;
+            cp_async16(sK + swz(row, c16, 8), k + base + (ok ? row * frame_stride : 0) + c16 * 8, ok);
+        }
+        cp_async_commit();
+#pragma unroll
+        for (int i = 0; i < kRows * 8 / 32; ++i) {
+            const int chunk = lane + 32 * i, row = chunk >> 3, c16 = chunk & 7;
+            const bool ok = row < T;
+            cp_async16(sV + swz(row, c16, 8), v + base + (ok ? row * frame_stride : 0) + c16 * 8, ok);
+        }
+        cp_async_commit();
+        for (int mt = 0; mt < kTiles; ++mt) {
+            // ---- Q (A fragments) of query frames 16 mt + g and 16 mt + g + 8, straight from global
+            const int q0 = 16 * mt + g, q1 = q0 + 8;
+            const bool r0 = q0 < T, r1 = q1 < T;
+            const __half* q0p = q + base + (long long)q0 * frame_stride;
+            const __half* q1p = q + base + (long long)q1 * frame_stride;
+            uint32_t qa[4][4];
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+                const int c = 16 * ks + 2 * t4;
+                qa[ks][0] = r0 ? *reinterpret_cast<const uint32_t*>(q0p + c) : 0u;
+                qa[ks][1] = r1 ? *reinterpret_cast<const uint32_t*>(q1p + c) : 0u;
+                qa[ks][2] = r0 ? *reinterpret_cast<const uint32_t*>(q0p + c + 8) : 0u;
+                qa[ks][3] = r1 ? *reinterpret_cast<const uint32_t*>(q1p + c + 8) : 0u;
+            }
+            if (mt == 0) {
+                cp_async_wait<1>();   // K has landed
+                __syncwarp();
+            }
+            // ---- S = Q K^T over all 16 kTiles keys (n tiles 2 np, 2 np + 1 from one ldmatrix.x4 per 16 d)
+            float sacc[2 * kTiles][4];
+#pragma unroll
+            for (int nt = 0; nt < 2 * kTiles; ++nt) sacc[nt][0] = sacc[nt][1] = sacc[nt][2] = sacc[nt][3] = 0.f;
+#pragma unroll
+            for (int np = 0; np < kTiles; ++np) {
+#pragma unroll
+                for (int ks = 0; ks < 4; ++ks) {
+                    uint32_t b0, b1, b2, b3;
+                    ldsm_x4(sK + swz(np * 16 + (lane & 7) + ((lane >> 4) << 3), 2 * ks + ((lane >> 3) & 1), 8), b0, b1,
+                            b2, b3);
+                    mma_m16n8k16(sacc[2 * np], qa[ks], b0, b1);
+                    mma_m16n8k16(sacc[2 * np + 1], qa[ks], b2, b3);
+                }
+            }
+            // ---- exact softmax over the T keys of rows g and g + 8 (a row lives in the 4 lanes of a quad)
+            float m0 = -INFINITY, m1 = -INFINITY;
+#pragma unroll
+            for (int nt = 0; nt < 2 * kTiles; ++nt) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const bool key_ok = (8 * nt + 2 * t4 + i) < T;
+                    sacc[nt][i] = key_ok ? sacc[nt][i] * scale_log2 : -INFINITY;
+                    sacc[nt][2 + i] = key_ok ? sacc[nt][2 + i] * scale_log2 : -INFINITY;
+                    m0 = fmaxf(m0, sacc[nt][i]);
+                    m1 = fmaxf(m1, sacc[nt][2 + i]);
+                }
+            }
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+            m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+            m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+            m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+            float l0 = 0.f, l1 = 0.f;
+#pragma unroll
+            for (int nt = 0; nt < 2 * kTiles; ++nt) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    sacc[nt][i] = exp2f(sacc[nt][i] - m0);
+                    sacc[nt][2 + i] = exp2f(sacc[nt][2 + i] - m1);
+                    l0 += sacc[nt][i];
+                    l1 += sacc[nt][2 + i];
+                }
+            }
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+            l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+            l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+            const float inv0 = 1.0f / l0, inv1 = 1.0f / l1;
+            // P = hi + lo, both fp16 (at most 64 keys per query: the fp16 rounding of P is not averaged away)
+            uint32_t pa[kTiles][4], pl[kTiles][4];
+#pragma unroll
+            for (int kb = 0; kb < kTiles; ++kb) {
+                split_h2(sacc[2 * kb][0] * inv0, sacc[2 * kb][1] * inv0, pa[kb][0], pl[kb][0]);
+                split_h2(sacc[2 * kb][2] * inv1, sacc[2 * kb][3] * inv1, pa[kb][1], pl[kb][1]);
+                split_h2(sacc[2 * kb + 1][0] * inv0, sacc[2 * kb + 1][1] * inv0, pa[kb][2], pl[kb][2]);
+                split_h2(sacc[2 * kb + 1][2] * inv1, sacc[2 * kb + 1][3] * inv1, pa[kb][3], pl[kb][3]);
+            }
+            if (mt == 0) {
+                cp_async_wait<0>();   // V has landed
+                __syncwarp();
+            }
+            // ---- O = P V, V fragments by ldmatrix.trans (two 8-wide d tiles per instruction)
+            __half* o0p = out + ((b * T + q0) * P + pix) * ldo + h * 64;
+            __half* o1p = out + ((b * T + q1) * P + pix) * ldo + h * 64;
+#pragma unroll
+            for (int nd = 0; nd < 8; nd += 2) {
+                float oa[4] = {0.f, 0.f, 0.f, 0.f}, ob[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+                for (int kb = 0; kb < kTiles; ++kb) {
+                    // lane i supplies the row address of matrix i/8: (k 0-7, nd), (k 8-15, nd), (k 0-7, nd+1), (k 8-15, nd+1)
+                    uint32_t b0, b1, b2, b3;
+                    ldsm_x4_t(sV + swz(16 * kb + (lane & 7) + ((lane >> 3) & 1) * 8, nd + (lane >> 4), 8), b0, b1, b2,
+                              b3);
+                    mma_m16n8k16(oa, pl[kb], b0, b1);
+                    mma_m16n8k16(ob, pl[kb], b2, b3);
+                    mma_m16n8k16(oa, pa[kb], b0, b1);
+                    mma_m16n8k16(ob, pa[kb], b2, b3);
+                }
+                if (r0) {
+                    *reinterpret_cast<uint32_t*>(o0p + 8 * nd + 2 * t4) = pack_h2(oa[0], oa[1]);
+                    *reinterpret_cast<uint32_t*>(o0p + 8 * (nd + 1) + 2 * t4) = pack_h2(ob[0], ob[1]);
+                }
+                if (r1) {
+                    *reinterpret_cast<uint32_t*>(o1p + 8 * nd + 2 * t4) = pack_h2(oa[2], oa[3]);
+                    *reinterpret_cast<uint32_t*>(o1p + 8 * (nd + 1) + 2 * t4) = pack_h2(ob[2], ob[3]);
+                }
+            }
+        }
+        __syncwarp();   // the smem K / V tiles are reused by the next item
     }
 }
 
@@ -667,11 +716,29 @@ extern "C" int tc_debug_read_attn_trace(unsigned long long* host_dst, int count)
     return fail(TC_ERR_INVALID, "tc_debug_read_attn_trace: the attention kernel records no timeline");
 }
 
+// 16 < T <= 64: kTiles = ceil(T / 16); 4 warps x (K + V) tiles of 16 kTiles rows x 128 bytes (up to 64 KiB)
+template <int kTiles>
+static int launch_temporal64(dim3 grid, cudaStream_t stream, const __half* q, const __half* k, const __half* v,
+                             long long ld, __half* out, long long ldo, int B, int T, int P, int heads, float sl2) {
+    constexpr int smem_bytes = 4 * 2 * kTiles * 16 * 128;
+    static bool attr_set = false;
+    if (!attr_set) {
+        int rc = check_cuda(cudaFuncSetAttribute(temporal_attn_mma64_kernel<kTiles>,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes),
+                            "cudaFuncSetAttribute(temporal_attn_mma64_kernel)");
+        if (rc) return rc;
+        attr_set = true;
+    }
+    tc_host::launch(temporal_attn_mma64_kernel<kTiles>, grid, dim3(128), smem_bytes, stream, 1, q, k, v, ld, out, ldo, B,
+                    T, P, heads, sl2);
+    return TC_OK;
+}
+
 extern "C" int tc_temporal_attention(const void* q, const void* k, const void* v, long long ld, void* out,
                                      long long ldo, int B, int T, int P, int heads, float scale, void* stream_v) {
     cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
     TC_CHECK_ARG(q && k && v && out, "tc_temporal_attention: null pointer");
-    TC_CHECK_ARG(B > 0 && T > 0 && T <= 32 && P > 0 && heads > 0, "tc_temporal_attention: need 0 < T <= 32");
+    TC_CHECK_ARG(B > 0 && T > 0 && T <= 64 && P > 0 && heads > 0, "tc_temporal_attention: need 0 < T <= 64");
     TC_CHECK_ARG(ld % 8 == 0 && ldo % 8 == 0, "tc_temporal_attention: strides must be multiples of 8");
     TC_CHECK_ARG(ld >= 64LL * heads && ldo >= 64LL * heads, "tc_temporal_attention: ld and ldo must be at least heads * 64");
     TC_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) | reinterpret_cast<uintptr_t>(v) |
@@ -682,15 +749,19 @@ extern "C" int tc_temporal_attention(const void* q, const void* k, const void* v
     const __half* kp = reinterpret_cast<const __half*>(k);
     const __half* vp = reinterpret_cast<const __half*>(v);
     __half* op = reinterpret_cast<__half*>(out);
-    if (T <= 16) {
-        long long blocks = (items + 3) / 4;
-        const long long cap = 16LL * sm_count();
-        if (blocks > cap) blocks = cap;
+    long long blocks = (items + 3) / 4;
+    const long long cap = 16LL * sm_count();
+    if (blocks > cap) blocks = cap;
+    int rc = TC_OK;
+    if (T <= 16)
         tc_host::launch(temporal_attn_mma_kernel, dim3((unsigned)blocks), dim3(128), 0, stream, 1, qp, kp, vp, ld, op, ldo, B, T, P, heads, sl2);
-    } else {
-        const long long blocks = (items + 3) / 4;
-        tc_host::launch(temporal_attn_kernel<32>, dim3((unsigned)blocks), dim3(128), 0, stream, 1, qp, kp, vp, ld, op, ldo, B, T, P, heads, sl2);
-    }
+    else if (T <= 32)
+        rc = launch_temporal64<2>(dim3((unsigned)blocks), stream, qp, kp, vp, ld, op, ldo, B, T, P, heads, sl2);
+    else if (T <= 48)
+        rc = launch_temporal64<3>(dim3((unsigned)blocks), stream, qp, kp, vp, ld, op, ldo, B, T, P, heads, sl2);
+    else
+        rc = launch_temporal64<4>(dim3((unsigned)blocks), stream, qp, kp, vp, ld, op, ldo, B, T, P, heads, sl2);
+    if (rc) return rc;
     count_launch();
     TC_CHECK_LAUNCH("temporal_attn_kernel");
     return TC_OK;

@@ -355,7 +355,8 @@ class UNetEngine(Engine):
             C = att.C
             segs = [dict(k=kv["txt"], v=kv["txt"], ldk=2 * C, ldv=2 * C, Lk=kv["n_txt"], kv_div=T, v_offset=C)]
             if kv["img"] is not None:
-                segs.append(dict(k=kv["img"], v=kv["img"], ldk=2 * C, ldv=2 * C, Lk=kv["n_img"], kv_div=1, v_offset=C))
+                segs.append(dict(k=kv["img"], v=kv["img"], ldk=2 * C, ldv=2 * C, Lk=kv["n_img"], kv_div=kv["img_div"],
+                                 v_offset=C))
             bld.op(ops.attention, q.t, segs, att.t, q_batches=att.N, Lq=att.H * att.W, heads=heads, scale=64 ** -0.5,
                    ldq=C, ldo=C)
 
@@ -397,9 +398,13 @@ class UNetEngine(Engine):
     def _build(self, B: int, T: int, H: int, W: int, n_ctx: int):
         lay, dev = self.lay, self.dev
         N = B * T
-        if n_ctx != 77 + 16 * T:
-            raise NotImplementedError("context must hold 77 text + 16 image tokens per frame "
-                                      "(openaimodel3d.py:556 hard-codes this layout)")
+        if n_ctx <= 77:
+            raise NotImplementedError("context must hold 77 text tokens and at least one image token")
+        # openaimodel3d.py:556-562: a context of exactly 77 + 16 T tokens gives frame t its own 16 image tokens (image
+        # K/V rows per frame); any other length gives every frame the whole context (image K/V rows per sample, shared
+        # by its T frames like the text rows)
+        per_frame = n_ctx == 77 + 16 * T
+        n_img, img_rows, img_div = (16, N * 16, 1) if per_frame else (n_ctx - 77, B * (n_ctx - 77), T)
         # arena: generous static budget (activations of one B-sample forward)
         px = N * H * W
         arena_bytes = self.arena_bytes or int(px * lay.model_channels * 2 * 40 + (256 << 20))
@@ -413,7 +418,7 @@ class UNetEngine(Engine):
         plan.t_in = torch.zeros(B, dtype=torch.float32, device=dev)
         plan.fs_in = torch.zeros(B, dtype=torch.float32, device=dev)
         plan.ctx_txt = torch.zeros(B * 77, lay.context_dim, dtype=torch.float16, device=dev)
-        plan.ctx_img = torch.zeros(N * 16, lay.context_dim, dtype=torch.float16, device=dev)
+        plan.ctx_img = torch.zeros(img_rows, lay.context_dim, dtype=torch.float16, device=dev)
         plan.emb = torch.zeros(B, lay.time_dim, dtype=torch.float32, device=dev)
         plan.emb_ws = torch.zeros(B * (lay.model_channels + lay.time_dim), dtype=torch.float32, device=dev)
         plan.emb_all = torch.zeros(B, self.emb_cols, dtype=torch.float16, device=dev)
@@ -433,7 +438,7 @@ class UNetEngine(Engine):
         kvs = {}
         cb = Builder(arena, ctxp)
         txt = Act(plan.ctx_txt, 1, 1, B * 77, lay.context_dim, lay.context_dim)
-        img = Act(plan.ctx_img, 1, 1, N * 16, lay.context_dim, lay.context_dim)
+        img = Act(plan.ctx_img, 1, 1, img_rows, lay.context_dim, lay.context_dim)
 
         def make_kv(p: _P):
             C = p.inner
@@ -441,9 +446,9 @@ class UNetEngine(Engine):
             linear(cb, txt, p.tb.kv_txt, Act(kt, 1, 1, B * 77, 2 * C, 2 * C))
             ki = None
             if p.tb.kv_img is not None:
-                ki = torch.zeros(N * 16, 2 * C, dtype=torch.float16, device=dev)
-                linear(cb, img, p.tb.kv_img, Act(ki, 1, 1, N * 16, 2 * C, 2 * C))
-            kvs[id(p)] = dict(txt=kt, img=ki, n_txt=77, n_img=16)
+                ki = torch.zeros(img_rows, 2 * C, dtype=torch.float16, device=dev)
+                linear(cb, img, p.tb.kv_img, Act(ki, 1, 1, img_rows, 2 * C, 2 * C))
+            kvs[id(p)] = dict(txt=kt, img=ki, n_txt=77, n_img=n_img, img_div=img_div)
 
         for blk in self.p_input + [self.p_middle] + self.p_output:
             for p in blk:
@@ -552,11 +557,11 @@ class UNetEngine(Engine):
         tensor (address, version counter, shape) identifies its CONTENT once an earlier tensor has been freed: the
         caching allocator hands the next `torch.cat` temporary the same block.  The program is 32 small GEMMs
         (< 0.2 ms) per call, against 50 denoising steps per `sample()`."""
-        B, T = plan.B, plan.T
+        B = plan.B
         if tuple(context.shape[:2]) != (B, plan.n_ctx):
             raise ValueError(f"context {tuple(context.shape)} does not fit the plan ({B}, {plan.n_ctx}, ...)")
         plan.ctx_txt.copy_(context[:, :77].reshape(B * 77, -1))
-        plan.ctx_img.copy_(context[:, 77:].reshape(B * T * 16, -1))
+        plan.ctx_img.copy_(context[:, 77:].reshape(plan.ctx_img.shape[0], -1))   # (b t) x 16 or b x (n_ctx - 77) rows
         self._execute(plan.ctx, executor)
 
     def load_inputs(self, plan, x, timesteps, fs) -> None:

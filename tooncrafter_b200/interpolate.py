@@ -9,7 +9,10 @@ With a single --frames image the image is animated instead (ToonCrafterPipeline.
         --frames still.png --height 576 --width 1024 --out results/clip
 
 Writes DIR/frame_%04d.png, DIR/video.npy (uint8 [F, H, W, 3]) and, when OpenCV can open an mp4 writer,
-DIR/video.mp4.  The sampling defaults are those of the reference's scripts/run.sh.
+DIR/video.mp4.  The sampling defaults are those of the reference's scripts/run.sh.  --video-length T sets the frames
+of each segment (the reference's --video_length; any even T from 4 to 64, default the config's temporal_length):
+
+    python -m tooncrafter_b200.interpolate --config ... --frames a.png b.png --video-length 32 --out results/long
 
 Under torchrun (WORLD_SIZE > 1) every process drives the GPU LOCAL_RANK over NCCL, builds the model (the checkpoint,
 or the same synthetic seed) and the segments are sharded over the processes (ToonCrafterPipeline's `group`);
@@ -61,6 +64,8 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--timestep-spacing", default="uniform_trailing")
     ap.add_argument("--segments-per-batch", type=int, default=None,
                     help="segments sampled together (default: 4 at 320x512, 1 at 576x1024)")
+    ap.add_argument("--video-length", type=int, default=None,
+                    help="frames per segment, an even number from 4 to 64 (default: the config's temporal_length)")
     ap.add_argument("--loop", action="store_true", help="add a closing segment from the last keyframe to the first")
     ap.add_argument("--seed", type=int, default=123)
     ap.add_argument("--latency-mode", action="store_true",
@@ -139,7 +144,14 @@ def write_video(video: np.ndarray, out_dir: str, fps: int) -> None:
 
 
 def main(argv=None) -> int:
-    args = get_parser().parse_args(argv)
+    ap = get_parser()
+    args = ap.parse_args(argv)
+    if args.video_length is not None:
+        from .pipeline import check_video_length
+        try:
+            check_video_length(args.video_length)
+        except ValueError as e:
+            ap.error(str(e))
     if not args.synthetic_weights and args.ckpt is None:
         raise SystemExit("give --ckpt, or --synthetic-weights for a run without a checkpoint")
     cfg = load_model_config(args.config, args.keep_config_targets)
@@ -177,7 +189,7 @@ def run(args, cfg, dev, group) -> int:
     pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
     common = dict(steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta, fs=args.frame_stride,
                   guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing, cfg_img=args.cfg_img,
-                  seed=args.seed, size=(args.height, args.width))
+                  seed=args.seed, size=(args.height, args.width), video_length=args.video_length)
     if len(frames) == 1:
         if args.loop:
             raise SystemExit("--loop needs at least two keyframes")

@@ -14,10 +14,10 @@ Per call:
   * ONE image-tower pass over the first keyframe of every segment plus the zero image, ONE text-tower pass over the
     distinct prompts plus "" (inference.py:186-216);
   * the segments as the batch rows of one fused DDIM sample() per group of `segments_per_batch`;
-  * per segment the T = 16 and T = 14 decodes (inference.py:262-270; one decode with a plain first stage, see below),
-    read in place by one tc_video_u8 launch that
-    applies the middle-frame splice and the uint8 conversion of the save path and writes the segment's frames into
-    the joined video at frame (T-1)*k.
+  * per segment the T and T - 2 decodes (inference.py:262-270; one decode with a plain first stage, see below), each
+    in chunks of en_and_decode_n_samples_a_time (default temporal_length) frames as decode_core runs them, read by one
+    tc_video_u8 launch that applies the middle-frame splice and the uint8 conversion of the save path and writes the
+    segment's frames into the joined video at frame (T-1)*k.
 
 RNG contract: keyframe j's posterior noise is drawn from a CPU generator seeded `seed + j`; segment k's x_T and
 DDIM step noise come from a generator on the model's device seeded `seed + k` (DDIMSampler's `noise_generators`).
@@ -31,9 +31,14 @@ video has (T-1)*S + 1 frames, or (T-1)*K with `loop`.
 `ToonCrafterPipeline.animate` is the same glue for one image (image_guided_synthesis with interp=False): one segment
 whose c_concat is the image's latent repeated over the T frames.
 
-First stage: with the dual-reference AutoencoderKL_Dualref each segment is decoded twice (T = 16 and T = 14, then
-spliced, as above).  The plain AutoencoderKL of the DynamiCrafter / training configs decodes every frame on its own, so
-each segment is decoded once, without reference maps, and tc_video_u8 runs without a splice.
+Clip length: `video_length` T (the reference's --video_length, inference.py:93-100, 197-203), any even T from 4 to 64,
+default the model's temporal_length.  The UNet gives each frame its own 16 image tokens only when the context holds
+77 + 16 T tokens; the pipeline's 77 + 256 tokens give every frame all of them at any other T (openaimodel3d.py:556-562).
+
+First stage: with the dual-reference AutoencoderKL_Dualref each segment is decoded twice (T and T - 2 frames, then
+spliced, as above), every chunk of frames with the segment's two reference maps.  The plain AutoencoderKL of the
+DynamiCrafter / training configs decodes every frame on its own, so each segment is decoded once, without reference
+maps, and tc_video_u8 runs without a splice.
 
 Several GPUs (`ToonCrafterPipeline(model, group)`, one process per GPU): the S segments are split into contiguous
 blocks by distributed.shard_clips, one block per rank, or one per GPU pair with `latency` (the pair samples its block
@@ -79,12 +84,40 @@ def preprocess(keyframes, size=(320, 512), device="cpu") -> torch.Tensor:
     return torch.stack(out).float().div(255).sub(0.5).div(0.5)
 
 
-def default_segments_per_batch(size) -> int:
+MIN_VIDEO_LENGTH, MAX_VIDEO_LENGTH = 4, 64
+
+
+def check_video_length(T) -> int:
+    """The clip lengths the pipeline runs: even (the interpolation video is T/2 copies of each keyframe,
+    inference.py:93-94), at least 4 (the middle-frame splice of the T - 2 decode), at most 64 (tc_temporal_attention)."""
+    if (isinstance(T, bool) or not isinstance(T, (int, np.integer)) or T % 2
+            or not MIN_VIDEO_LENGTH <= T <= MAX_VIDEO_LENGTH):
+        raise ValueError(f"video_length must be an even integer from {MIN_VIDEO_LENGTH} to {MAX_VIDEO_LENGTH}, got {T!r}")
+    return int(T)
+
+
+def default_segments_per_batch(size, T: int = 16) -> int:
     """Segments sampled together by default: as many as keep the UNet program at the activation budget of 4 segments
-    at 320 x 512 (8 rows of a 40 x 64 latent, an arena of about 8 GB; it grows with rows x latent pixels).  At
-    576 x 1024 that is 1 segment: with 4 the UNet arena alone would take 28 GiB, and a default call after an animate
-    call (whose plans stay cached) no longer fits on an 80 GB H100."""
-    return max(1, (4 * 320 * 512) // (size[0] * size[1]))
+    of 16 frames at 320 x 512 (8 rows of 16 frames of a 40 x 64 latent, an arena of about 8 GB; it grows with rows x
+    frames x latent pixels).  At 576 x 1024 and T = 16 that is 1 segment: with 4 the UNet arena alone would take 28 GiB,
+    and a default call after an animate call (whose plans stay cached) no longer fits on an 80 GB H100."""
+    return max(1, (4 * 16 * 320 * 512) // (T * size[0] * size[1]))
+
+
+def _decode_chunks(dec, lat, n: int, ref, ex):
+    """decode_core's loop (ddpm3d.py:656-675): lat [T, 4, h, w] decoded n frames at a time (a dual-reference decoder
+    with timesteps = the chunk's length and the same reference maps `ref`).  One chunk returns the plan's output view
+    as it is; several are copied into one [T, 3, H, W] tensor, since chunks of one length share a plan."""
+    args = () if ref is None else (ref,)
+    if lat.shape[0] <= n:
+        return dec.decode(lat.float(), *args, executor=ex)
+    out = None
+    for i in range(0, lat.shape[0], n):
+        y = dec.decode(lat[i:i + n].float(), *args, executor=ex)
+        if out is None:
+            out = torch.empty((lat.shape[0],) + tuple(y.shape[1:]), dtype=y.dtype, device=y.device)
+        out[i:i + y.shape[0]].copy_(y)
+    return out
 
 
 class ToonCrafterPipeline:
@@ -135,18 +168,22 @@ class ToonCrafterPipeline:
     def interpolate(self, keyframes, prompts: Union[str, Sequence[str], torch.Tensor] = "", steps: int = 50,
                     cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                     timestep_spacing: str = "uniform_trailing", cfg_img=None, loop: bool = False, seed: int = 123,
-                    size=(320, 512), segments_per_batch: Optional[int] = None, output: str = "uint8") -> torch.Tensor:
+                    size=(320, 512), segments_per_batch: Optional[int] = None, output: str = "uint8",
+                    video_length: Optional[int] = None) -> torch.Tensor:
         """keyframes: K >= 2 uint8 RGB images (tensor [K, H, W, 3], ndarray, or a list of [H, W, 3] arrays of any
         size).  prompts: one string for every segment, a list of S strings, or token ids [S, 77] (strings other than
         "" need open_clip's tokenizer).  cfg_img not None: three-way guidance (DDIMSamplerMultiCond).  Defaults are
         those of the reference's scripts/run.sh.
 
-        segments_per_batch None: default_segments_per_batch(size), 4 at 320 x 512 and 1 at 576 x 1024.
+        video_length: T frames per segment, an even number from 4 to 64 (ValueError otherwise); None: the model's
+        temporal_length.  segments_per_batch None: default_segments_per_batch(size, T), 4 at 320 x 512 and 1 at
+        576 x 1024 for T = 16.
 
         Returns uint8 [F, size[0], size[1], 3] on the model's device, F = (T-1)*S + 1 (or (T-1)*K with `loop`); with
         output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]]."""
+        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
         if segments_per_batch is None:
-            segments_per_batch = default_segments_per_batch(size)
+            segments_per_batch = default_segments_per_batch(size, T)
         frames = self._preprocess(keyframes, size, output)
         K = frames.shape[0]
         if K < 2:
@@ -154,25 +191,27 @@ class ToonCrafterPipeline:
         S = K if loop else K - 1
         return self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, steps, cfg_scale,
                               eta, fs, guidance_rescale, timestep_spacing, cfg_img, loop, seed, size,
-                              segments_per_batch, output)
+                              segments_per_batch, output, T)
 
     @torch.no_grad()
     def animate(self, image, prompt: Union[str, torch.Tensor] = "", steps: int = 50, cfg_scale: float = 7.5,
                 eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                 timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
-                output: str = "uint8") -> torch.Tensor:
+                output: str = "uint8", video_length: Optional[int] = None) -> torch.Tensor:
         """One image -> one T-frame video: image_guided_synthesis with interp=False, loop=False (inference.py:
         180-277; c_concat is the image's latent repeated over the T frames, :201-203), the image-to-video mode of
         the DynamiCrafter checkpoints.  image: a uint8 [H, W, 3] RGB image of any size; prompt: a string or token
         ids [1, 77].  The image's posterior noise comes from a CPU generator seeded `seed`, x_T and the DDIM step
         noise from a generator on the model's device seeded `seed` (keyframe 0 / segment 0 of `interpolate`); a
-        dual-reference first stage gets the image's encoder maps as both reference frames.
+        dual-reference first stage gets the image's encoder maps as both reference frames.  video_length: T, as for
+        interpolate.
 
         Returns uint8 [T, size[0], size[1], 3] on the model's device; with output="float", the spliced video before
         quantisation, float32 [3, T, size[0], size[1]]."""
+        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
         frames = self._preprocess([image], size, output)
         video = self._generate(frames, prompt, [0], [0], False, steps, cfg_scale, eta, fs, guidance_rescale,
-                               timestep_spacing, cfg_img, False, seed, size, 1, output)
+                               timestep_spacing, cfg_img, False, seed, size, 1, output, T)
         return video[0] if output == "float" else video
 
     def _preprocess(self, images, size, output) -> torch.Tensor:
@@ -184,14 +223,11 @@ class ToonCrafterPipeline:
             raise ValueError(f"size {tuple(size)} must be a multiple of 16")
         if m.model.conditioning_key != "hybrid":
             raise NotImplementedError("image-conditioned synthesis needs the hybrid (concat + cross-attention) model")
-        T = m.temporal_length
-        if (m.en_and_decode_n_samples_a_time or T) < T:
-            raise NotImplementedError("the pipeline decodes each segment's T frames in one call")
         return preprocess(images, size, m.device)
 
     def _generate(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
-                  timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output) -> torch.Tensor:
-        """S = len(first) segments; segment k runs from keyframe first[k] to keyframe last[k] (interp), or animates
+                  timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, T) -> torch.Tensor:
+        """S = len(first) segments of T frames; segment k runs from keyframe first[k] to keyframe last[k] (interp), or animates
         keyframe first[k] (not interp).  With a group, this rank computes its block of segments and the blocks are
         then broadcast."""
         if self.latency:
@@ -201,7 +237,6 @@ class ToonCrafterPipeline:
             if cfg_scale == 1.0:
                 raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
                                  "cfg_scale 1.0 has no unconditional branch")
-        T = self.model.temporal_length
         S = len(first)
         F = (T - 1) * S + (0 if loop else 1)
         video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=self.model.device) if output == "uint8"
@@ -209,7 +244,7 @@ class ToonCrafterPipeline:
         mine = list(range(S)) if self.group is None else distributed.shard_clips(S, self._block, self._n_blocks)
         if mine:
             self._render(frames, prompts, first, last, interp, steps, cfg_scale, eta, fs, guidance_rescale,
-                         timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video)
+                         timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video, T)
         if self.group is None:
             return video
         blocks = []
@@ -227,11 +262,11 @@ class ToonCrafterPipeline:
         return video
 
     def _render(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
-                timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video) -> None:
+                timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video, T) -> None:
         """Sample and decode segments `mine` (of S = len(first)) into their places in `video`."""
         m = self.model
         dev = m.device
-        T = m.temporal_length
+        n_dec = m.en_and_decode_n_samples_a_time or m.temporal_length                # decode_core's chunk
         ex = runtime.TEST_EXECUTOR
         K, S = frames.shape[0], len(first)
 
@@ -291,14 +326,14 @@ class ToonCrafterPipeline:
                 lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
                 if dual_ref:
                     ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
-                    y16 = dec.decode(lat.float(), ref, executor=ex)                     # views of the plans' outputs
-                    y14 = dec.decode(lat[keep].float(), ref, executor=ex)
+                    y16 = _decode_chunks(dec, lat, n_dec, ref, ex)      # a view of the plan's output for T <= n_dec
+                    y14 = _decode_chunks(dec, lat[keep], n_dec, ref, ex)
                 else:
                     # A frame-independent decoder turns each latent into the same frame whichever chunk holds it, so
                     # the reference's T - 2 pass is y16[keep] and the T - 2 decode is skipped.  For T >= 6 the two
                     # spliced frames (keep[T/2-2], keep[T/2-1] = latents T/2-1, T/2) are the frames already in place:
                     # no splice at all (tc_video_u8 with x14 = NULL).
-                    y16 = dec.decode(lat.float(), executor=ex)
+                    y16 = _decode_chunks(dec, lat, n_dec, None, ex)
                     y14 = None if T >= 6 else y16[keep]
                 if output == "float":
                     v = y16.float()
