@@ -32,6 +32,18 @@ device synchronise; the time reported is the maximum over ranks.
     torchrun --nproc-per-node 2 scripts/bench_pipeline.py --gpus 2 [--latency-mode]
     torchrun --nproc-per-node 2 scripts/bench_pipeline.py --gpus 2 --latency-mode --animate --first-stage plain \
         --size 576 1024
+
+--n-samples N [N ...] measures variants of a K = 2 interpolate() at --size, for each n in turn: one batched call
+(interpolate(n_samples=n), the variants as rows of the same sample() calls) against n separate single-sample calls,
+alternating; seconds per call and per sample, and the peak device memory of each arm (warm-up at DDIM-2):
+
+    python scripts/bench_pipeline.py --n-samples 1 2 4 8
+
+--pairs P measures interpolate_pairs() on P synthetic keyframe pairs (--n-samples n, default 1), sharded over --gpus
+N as above (the maximum over ranks): seconds per call and per clip:
+
+    python scripts/bench_pipeline.py --pairs 8 --gpus 1
+    torchrun --nproc-per-node 2 scripts/bench_pipeline.py --pairs 8 --gpus 2
 """
 from __future__ import annotations
 
@@ -190,6 +202,42 @@ def bench_video_length(args, model, info, build_s):
     return 0
 
 
+def bench_n_samples(args, model, info, build_s):
+    """K = 2 interpolate with n variants, batched against n single-sample calls (see the module docstring)."""
+    from tooncrafter_b200.pipeline import ToonCrafterPipeline
+    size = tuple(args.size)
+    pipe = ToonCrafterPipeline(model)
+    kf = (torch.rand(2, size[0], size[1], 3, generator=torch.Generator().manual_seed(0)) * 255).to(torch.uint8)
+    rows = []
+    for n in args.n_samples:
+        arms = dict(batched=lambda st: pipe.interpolate(kf, steps=st, seed=123, size=size, n_samples=n),
+                    separate=lambda st: [pipe.interpolate(kf, steps=st, seed=123 + v, size=size) for v in range(n)])
+        for fn in arms.values():
+            fn(2)
+        times, peaks = {a: [] for a in arms}, {a: 0 for a in arms}
+        for _ in range(args.reps):
+            for name, fn in arms.items():
+                dt, pk = _timed(lambda: fn(args.ddim_steps))
+                times[name].append(dt)
+                peaks[name] = max(peaks[name], pk)
+        row = dict(n_samples=n)
+        for name in arms:
+            best = min(times[name])
+            row[name] = dict(sec_per_call=best, sec_per_sample=best / n, all_s=[round(x, 3) for x in times[name]],
+                             peak_gib=peaks[name] / 2 ** 30)
+        row["batched_over_separate_time"] = row["batched"]["sec_per_call"] / row["separate"]["sec_per_call"]
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    out = dict(metric="K = 2 interpolation, n variants: seconds per call and per sample, batched vs n single-sample "
+               "calls (%dx%d, DDIM-%d, CFG 7.5, eta 1, synthetic weights, %s first stage)"
+               % (size[0], size[1], args.ddim_steps, args.first_stage), gpu=info, reps=args.reps,
+               model_build_s=build_s, configs=rows,
+               note="sec_per_call = best of the timed reps, host clock around work ending in a device synchronise; "
+                    "peak_gib = torch.cuda.max_memory_allocated over a timed call (model and cached plans included)")
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def bench_sharded(args, model, info, build_s, group):
     """--gpus N: K = 5 interpolate (or animate) sharded over `group` (None: one GPU); see the module docstring."""
     import torch.distributed as dist
@@ -200,7 +248,13 @@ def bench_sharded(args, model, info, build_s, group):
     pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
     g = torch.Generator().manual_seed(0)
     kf = (torch.rand(5, size[0], size[1], 3, generator=g) * 255).to(torch.uint8)
-    if args.animate:
+    if args.pairs is not None:
+        n = args.n_samples[0] if args.n_samples else 1
+        kp = (torch.rand(2 * args.pairs, size[0], size[1], 3, generator=g) * 255).to(torch.uint8)
+        pairs = [(kp[2 * i], kp[2 * i + 1]) for i in range(args.pairs)]
+        fn = lambda st: pipe.interpolate_pairs(pairs, n_samples=n, steps=st, seed=123, size=size)   # noqa: E731
+        frames, what = 16 * n * args.pairs, f"interpolate_pairs P={args.pairs} n={n}"
+    elif args.animate:
         fn, frames, what = (lambda st: pipe.animate(kf[0], steps=st, seed=123, size=size)), 16, "animate"
     else:
         fn, frames, what = (lambda st: pipe.interpolate(kf, steps=st, seed=123, size=size)), 15 * 4 + 1, "K=5"
@@ -222,6 +276,7 @@ def bench_sharded(args, model, info, build_s, group):
                                  "s" if args.gpus > 1 else "", size[0], size[1], args.ddim_steps, args.first_stage),
                gpu=info, gpus=args.gpus, latency_mode=args.latency_mode, reps=args.reps, model_build_s=build_s,
                frames=frames, sec_per_video=best, frames_per_s=frames / best, all_s=[round(x, 3) for x in times],
+               **(dict(pairs=args.pairs, sec_per_clip=best * 16 / frames) if args.pairs is not None else {}),
                note="sec_per_video = best of the timed reps; each rep is the maximum over ranks of a host clock "
                     "started after a barrier and stopped after a device synchronise")
     print(json.dumps(out), flush=True)
@@ -241,7 +296,14 @@ def main():
     ap.add_argument("--latency-mode", action="store_true", help="with --gpus: one clip per GPU pair")
     ap.add_argument("--video-length", type=int, nargs="+", default=None, metavar="T",
                     help="measure K = 2 interpolation at each of these frames-per-segment counts (docstring)")
+    ap.add_argument("--n-samples", type=int, nargs="+", default=None, metavar="N",
+                    help="measure K = 2 interpolation with each of these numbers of variants (docstring); with "
+                         "--pairs, the variants per pair")
+    ap.add_argument("--pairs", type=int, default=None, metavar="P",
+                    help="measure interpolate_pairs on P synthetic pairs over --gpus N (default 1)")
     args = ap.parse_args()
+    if args.pairs is not None and args.gpus is None:
+        args.gpus = 1
     if args.video_length is not None:
         from tooncrafter_b200.pipeline import check_video_length
         try:
@@ -284,6 +346,8 @@ def main():
         return bench_animate(args, model, info, build_s, decode16)
     if args.video_length is not None:
         return bench_video_length(args, model, info, build_s)
+    if args.n_samples is not None:
+        return bench_n_samples(args, model, info, build_s)
     pipe = ToonCrafterPipeline(model)
     g = torch.Generator().manual_seed(0)
     results = []

@@ -20,6 +20,15 @@ or the same synthetic seed) and the segments are sharded over the processes (Too
 
     torchrun --nproc-per-node 8 -m tooncrafter_b200.interpolate --config ... --frames a.png b.png c.png --out DIR
 
+--n-samples N makes N variants (the reference's --n_samples; ToonCrafterPipeline's n_samples) and writes variant v to
+DIR/sample{v}/.  --prompt-dir SRC instead of --frames runs a directory of independent keyframe pairs as the
+reference's --prompt_dir with --interp does (read_prompt_dir): pair i is the sorted images 2i and 2i+1 with line i of
+the directory's first .txt file (or "" without --text-input), and variant v of pair i goes to
+DIR/<name of image 2i>_sample{v}/ (ToonCrafterPipeline.interpolate_pairs, pair i seeded seed + i):
+
+    python -m tooncrafter_b200.interpolate --config ... --ckpt ... --prompt-dir prompts/512_interp --n-samples 4 \
+        --out results/
+
 The config is the reference-style YAML (read with PyYAML; only its `model:` section is used, so the training
 configs, whose first stage is the plain AutoencoderKL, work as well).  Its two OpenCLIP conditioning targets
 (lvdm.modules.encoders.condition.FrozenOpenCLIP*) are pointed at this repository's classes unless
@@ -28,6 +37,7 @@ configs, whose first stage is the plain AutoencoderKL, work as well).  Its two O
 from __future__ import annotations
 
 import argparse
+import glob
 import os
 import sys
 
@@ -48,8 +58,16 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--synthetic-weights", action="store_true", help="seeded synthetic weights instead of --ckpt")
     ap.add_argument("--keep-config-targets", action="store_true",
                     help="keep the YAML's OpenCLIP targets instead of this repository's classes")
-    ap.add_argument("--frames", nargs="+", required=True,
-                    help="K >= 2 keyframe images, in order; one image: animate it")
+    src = ap.add_mutually_exclusive_group(required=True)
+    src.add_argument("--frames", nargs="+", help="K >= 2 keyframe images, in order; one image: animate it")
+    src.add_argument("--prompt-dir", default=None,
+                     help="a directory of keyframe pairs and a prompt file, laid out as the reference's --prompt_dir")
+    ap.add_argument("--text-input", action="store_true",
+                    help="with --prompt-dir: pair i gets line i of the prompt file (default: every pair gets \"\")")
+    ap.add_argument("--n-samples", type=int, default=None,
+                    help="variants per video, written to OUT/sample{v}/ (OUT/<name>_sample{v}/ with --prompt-dir)")
+    ap.add_argument("--pairs-per-batch", type=int, default=None,
+                    help="with --prompt-dir: pairs sampled together (default: as many as the rows budget allows)")
     ap.add_argument("--prompt", default="", help="prompt of every segment")
     ap.add_argument("--prompts-file", default=None, help="one prompt per segment, one per non-empty line")
     ap.add_argument("--out", required=True, help="output directory")
@@ -111,6 +129,45 @@ def load_checkpoint(model, path: str) -> None:
         raise RuntimeError("\n".join(msg))
 
 
+IMAGE_SUFFIXES = ("jpg", "png", "jpeg", "JPEG", "PNG")
+
+
+def _filelist(data_dir: str, postfixes) -> list:
+    """get_filelist (inference.py:19-25): the files matching each `*.{postfix}`, collected and then sorted."""
+    files = []
+    for postfix in postfixes:
+        files.extend(glob.glob(os.path.join(data_dir, f"*.{postfix}")))
+    files.sort()
+    return files
+
+
+def read_prompt_dir(data_dir: str, text_input: bool = False):
+    """A --prompt_dir of the reference for interpolation (load_data_prompts with interp, inference.py:54-106).
+
+    Prompts: the non-empty stripped lines of the first `.txt` file by name; P = their number.  Images: the files
+    `*.jpg|png|jpeg|JPEG|PNG`, sorted as get_filelist sorts them; pair i is images 2i and 2i+1.  A pair's prompt is its
+    line with text_input and "" without (inference.py:186-187).  Its output name is image 2i's file name up to the
+    first dot, as save_results_seperate names `<name>_sample{v}.mp4`.  Returns ([(image a, image b)], prompts, names);
+    ValueError for a missing directory or prompt file, no prompts, or fewer than 2P images."""
+    if not os.path.isdir(data_dir):
+        raise ValueError(f"{data_dir}: not a directory")
+    txt = _filelist(data_dir, ["txt"])
+    if not txt:
+        raise ValueError(f"{data_dir}: no prompt file (*.txt)")
+    with open(txt[0]) as f:
+        lines = [ln.strip() for ln in f if ln.strip()]
+    if not lines:
+        raise ValueError(f"{txt[0]}: no prompts")
+    images = _filelist(data_dir, IMAGE_SUFFIXES)
+    P = len(lines)
+    if len(images) < 2 * P:
+        raise ValueError(f"{data_dir}: {len(images)} images for {P} prompts; pair i is images 2i and 2i+1, so "
+                         f"{2 * P} are needed")
+    pairs = [(images[2 * i], images[2 * i + 1]) for i in range(P)]
+    names = [os.path.basename(a).split(".")[0] for a, _ in pairs]
+    return pairs, (lines if text_input else [""] * P), names
+
+
 def read_prompts(args, n_segments: int):
     if args.prompts_file is None:
         return args.prompt
@@ -146,12 +203,27 @@ def write_video(video: np.ndarray, out_dir: str, fps: int) -> None:
 def main(argv=None) -> int:
     ap = get_parser()
     args = ap.parse_args(argv)
-    if args.video_length is not None:
-        from .pipeline import check_video_length
-        try:
+    from .pipeline import check_n_samples, check_video_length
+    try:
+        if args.video_length is not None:
             check_video_length(args.video_length)
+        if args.n_samples is not None:
+            check_n_samples(args.n_samples)
+        if args.pairs_per_batch is not None and args.pairs_per_batch < 1:
+            raise ValueError(f"--pairs-per-batch must be at least 1, got {args.pairs_per_batch}")
+    except ValueError as e:
+        ap.error(str(e))
+    if args.prompt_dir is not None:
+        if args.loop:
+            ap.error("--loop does not apply to --prompt-dir")
+        if args.prompt or args.prompts_file:
+            ap.error("--prompt-dir reads its prompts from the directory's .txt file (--prompt / --prompts-file)")
+        try:
+            read_prompt_dir(args.prompt_dir, args.text_input)
         except ValueError as e:
             ap.error(str(e))
+    elif args.text_input or args.pairs_per_batch is not None:
+        ap.error("--text-input and --pairs-per-batch apply to --prompt-dir")
     if not args.synthetic_weights and args.ckpt is None:
         raise SystemExit("give --ckpt, or --synthetic-weights for a run without a checkpoint")
     cfg = load_model_config(args.config, args.keep_config_targets)
@@ -185,25 +257,63 @@ def run(args, cfg, dev, group) -> int:
         load_checkpoint(model, args.ckpt)
         model = model.to(dev).eval()
     model.perframe_ae = True
-    frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
     pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
     common = dict(steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta, fs=args.frame_stride,
                   guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing, cfg_img=args.cfg_img,
-                  seed=args.seed, size=(args.height, args.width), video_length=args.video_length)
+                  size=(args.height, args.width), video_length=args.video_length)
+    writes = group is None or torch.distributed.get_rank() == 0
+    if args.prompt_dir is not None:
+        return run_prompt_dir(args, pipe, common, group, writes)
+    frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
     if len(frames) == 1:
         if args.loop:
             raise SystemExit("--loop needs at least two keyframes")
-        video = pipe.animate(frames[0], prompt=read_prompts(args, 1), **common)
+        video = pipe.animate(frames[0], prompt=read_prompts(args, 1), seed=args.seed, n_samples=args.n_samples,
+                             **common)
     else:
         n_seg = len(frames) if args.loop else len(frames) - 1
-        video = pipe.interpolate(frames, prompts=read_prompts(args, n_seg), loop=args.loop,
-                                 segments_per_batch=args.segments_per_batch, **common)
-    if group is not None and torch.distributed.get_rank() != 0:
+        video = pipe.interpolate(frames, prompts=read_prompts(args, n_seg), loop=args.loop, seed=args.seed,
+                                 segments_per_batch=args.segments_per_batch, n_samples=args.n_samples, **common)
+    if not writes:
         return 0
     v = video.cpu().numpy()
-    write_video(v, args.out, args.fps)
-    print(f"{len(frames)} {'image' if len(frames) == 1 else 'keyframes'} -> {v.shape[0]} frames of "
-          f"{v.shape[1]}x{v.shape[2]} in {args.out}")
+    if args.n_samples is None:
+        write_video(v, args.out, args.fps)
+    else:
+        for i, variant in enumerate(v):
+            write_video(variant, os.path.join(args.out, f"sample{i}"), args.fps)
+    print(f"{len(frames)} {'image' if len(frames) == 1 else 'keyframes'} -> "
+          f"{'' if args.n_samples is None else f'{v.shape[0]} x '}{v.shape[-4]} frames of {v.shape[-3]}x{v.shape[-2]} "
+          f"in {args.out}")
+    return 0
+
+
+def run_prompt_dir(args, pipe, common, group, writes: bool) -> int:
+    """--prompt-dir: the directory's pairs through interpolate_pairs in chunks of (blocks x pairs per batch) pairs,
+    each chunk written before the next is read, so host and device memory hold one chunk; pair i is seeded seed + i
+    whatever chunk holds it.  Every pair runs (the reference drops the P % ranks pairs left over)."""
+    from PIL import Image
+
+    from .pipeline import check_video_length, default_pairs_per_batch
+    pairs, prompts, names = read_prompt_dir(args.prompt_dir, args.text_input)
+    n = 1 if args.n_samples is None else args.n_samples
+    T = check_video_length(pipe.model.temporal_length if args.video_length is None else args.video_length)
+    per_batch = args.pairs_per_batch or default_pairs_per_batch(common["size"], T, n)
+    blocks = 1 if group is None else torch.distributed.get_world_size(group) // (2 if args.latency_mode else 1)
+    chunk = blocks * per_batch
+    for c0 in range(0, len(pairs), chunk):
+        idx = range(c0, min(c0 + chunk, len(pairs)))
+        images = [[np.asarray(Image.open(p).convert("RGB")) for p in pairs[i]] for i in idx]
+        video = pipe.interpolate_pairs(images, prompts=[prompts[i] for i in idx], n_samples=n, seed=args.seed + c0,
+                                       pairs_per_batch=per_batch, **common)
+        if not writes:
+            continue
+        v = video.cpu().numpy()
+        for j, i in enumerate(idx):
+            for s in range(n):
+                write_video(v[j, s], os.path.join(args.out, f"{names[i]}_sample{s}"), args.fps)
+    if writes:
+        print(f"{len(pairs)} pairs x {n} samples from {args.prompt_dir} -> {args.out}")
     return 0
 
 

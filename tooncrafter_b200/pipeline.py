@@ -24,6 +24,20 @@ DDIM step noise come from a generator on the model's device seeded `seed + k` (D
 So segment k of a K-keyframe run is the same computation as a 2-keyframe run on (keyframe k, keyframe k+1) with
 `seed + k`, whatever batch it runs in (up to the batch tiling of the kernels).
 
+Variants (`n_samples`, the reference's --n_samples, image_guided_synthesis's loop at inference.py:234-274): n videos
+that share the keyframe latents (the posterior noise above, drawn once), the tower outputs and the decoder reference
+maps, and differ only in their DDIM noise: variant v of segment k draws from a device generator seeded
+`seed + k + v * VARIANT_SEED_STRIDE` (2**32 + 0x9E3779B9), so variant 0 is the single-sample video and the seed of
+(k, v) depends neither on n, S, the batch nor the rank.  A sampled row is one (segment, variant); rows run in variant-major order r = v * S + k, so
+`segments_per_batch` consecutive rows share a sample() call and a contiguous block of rows writes a contiguous range
+of the flattened [n * F] video (of [n * S] segments for float output).
+
+Pair directories (`interpolate_pairs`, the reference's --prompt_dir with --interp, inference.py:64-106 and 280-340):
+P independent pairs, pair i being the call interpolate([a_i, b_i], prompts=p_i, seed=seed + i, n_samples=n,
+segments_per_batch=n).  Pairs are taken `pairs_per_batch` at a time, each group encoded, conditioned and sampled on
+its own (pair-major rows, pair i's variant v being row i * n + v); with one pair per group the call is therefore
+bit for bit that sequence of interpolate calls, and memory does not grow with P.
+
 Seam rule: neighbouring segments share a keyframe; the earlier segment's last frame is kept and the later segment's
 frame 0 is dropped.  With `loop`, the closing segment's last frame (keyframe 0 again) is dropped as well, so the
 video has (T-1)*S + 1 frames, or (T-1)*K with `loop`.
@@ -40,13 +54,14 @@ spliced, as above), every chunk of frames with the segment's two reference maps.
 DynamiCrafter / training configs decodes every frame on its own, so each segment is decoded once, without reference
 maps, and tc_video_u8 runs without a splice.
 
-Several GPUs (`ToonCrafterPipeline(model, group)`, one process per GPU): the S segments are split into contiguous
+Several GPUs (`ToonCrafterPipeline(model, group)`, one process per GPU): the n * S rows are split into contiguous
 blocks by distributed.shard_clips, one block per rank, or one per GPU pair with `latency` (the pair samples its block
 with DDIMSampler.latency_group, one guidance branch per GPU, and pair-rank 0 decodes).  Every rank still encodes all
 K keyframes and runs the two conditioning towers over the inputs of the single-process call, then takes its own
 rows: the batch sizes, and with them the kernels' tiling, are those of the single-process call.  By the RNG contract a
-segment is then the same computation whichever rank runs it; each block writes its contiguous range of the joined
-video, and the blocks are broadcast so that every rank returns the full video.
+row is then the same computation whichever rank runs it; each block writes its contiguous range of the flattened
+video, and the blocks are broadcast so that every rank returns the full result.  interpolate_pairs splits the P pairs
+the same way (each rank encoding only its own groups) and broadcasts each block's pairs.
 """
 from __future__ import annotations
 
@@ -102,6 +117,26 @@ def default_segments_per_batch(size, T: int = 16) -> int:
     frames x latent pixels).  At 576 x 1024 and T = 16 that is 1 segment: with 4 the UNet arena alone would take 28 GiB,
     and a default call after an animate call (whose plans stay cached) no longer fits on an 80 GB H100."""
     return max(1, (4 * 16 * 320 * 512) // (T * size[0] * size[1]))
+
+
+def default_pairs_per_batch(size, T: int, n_samples: int) -> int:
+    """interpolate_pairs' default group: as many pairs as keep its pairs x n_samples rows within
+    default_segments_per_batch(size, T), and at least one (a pair's variants always share one sample() call)."""
+    return max(1, default_segments_per_batch(size, T) // n_samples)
+
+
+# Variant v of a row whose single-sample noise seed is s draws from a generator seeded s + v * VARIANT_SEED_STRIDE: far
+# from the seeds seed + k of the other segments (and pairs), and independent of the number of variants or rows.  The
+# stride is 2**32 plus the 32-bit golden-ratio constant, so that variants differ in the low 32 bits as well: a CUDA
+# generator keeps all 64 bits of its seed, a CPU generator (mt19937) only the low 32.
+VARIANT_SEED_STRIDE = 2 ** 32 + 0x9E3779B9
+
+
+def check_n_samples(n) -> int:
+    """Variants per input (the reference's --n_samples): an integer >= 1; bools are refused."""
+    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 1:
+        raise ValueError(f"n_samples must be an integer >= 1, got {n!r}")
+    return int(n)
 
 
 def _decode_chunks(dec, lat, n: int, ref, ex):
@@ -169,19 +204,24 @@ class ToonCrafterPipeline:
                     cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                     timestep_spacing: str = "uniform_trailing", cfg_img=None, loop: bool = False, seed: int = 123,
                     size=(320, 512), segments_per_batch: Optional[int] = None, output: str = "uint8",
-                    video_length: Optional[int] = None) -> torch.Tensor:
+                    video_length: Optional[int] = None, n_samples: Optional[int] = None) -> torch.Tensor:
         """keyframes: K >= 2 uint8 RGB images (tensor [K, H, W, 3], ndarray, or a list of [H, W, 3] arrays of any
         size).  prompts: one string for every segment, a list of S strings, or token ids [S, 77] (strings other than
         "" need open_clip's tokenizer).  cfg_img not None: three-way guidance (DDIMSamplerMultiCond).  Defaults are
         those of the reference's scripts/run.sh.
 
         video_length: T frames per segment, an even number from 4 to 64 (ValueError otherwise); None: the model's
-        temporal_length.  segments_per_batch None: default_segments_per_batch(size, T), 4 at 320 x 512 and 1 at
-        576 x 1024 for T = 16.
+        temporal_length.  n_samples: None, or n >= 1 variants of the whole video (the reference's --n_samples), which
+        share the keyframe latents, the conditioning and the decoder reference maps and differ in their DDIM noise
+        only (module docstring).  segments_per_batch: sampled rows, one (segment, variant) each, per sample() call;
+        None: default_segments_per_batch(size, T), 4 at 320 x 512 and 1 at 576 x 1024 for T = 16.
 
         Returns uint8 [F, size[0], size[1], 3] on the model's device, F = (T-1)*S + 1 (or (T-1)*K with `loop`); with
-        output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]]."""
+        output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]].
+        With an integer n_samples both gain a leading variant axis, [n, F, H, W, 3] / [n, S, 3, T, H, W], and
+        video[v] is a complete single-sample result (video[0] is the n_samples=None result)."""
         T = check_video_length(self.model.temporal_length if video_length is None else video_length)
+        n = 1 if n_samples is None else check_n_samples(n_samples)
         if segments_per_batch is None:
             segments_per_batch = default_segments_per_batch(size, T)
         frames = self._preprocess(keyframes, size, output)
@@ -189,89 +229,183 @@ class ToonCrafterPipeline:
         if K < 2:
             raise ValueError("interpolation needs at least two keyframes")
         S = K if loop else K - 1
-        return self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, steps, cfg_scale,
-                              eta, fs, guidance_rescale, timestep_spacing, cfg_img, loop, seed, size,
-                              segments_per_batch, output, T)
+        video = self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, loop, seed, n,
+                               segments_per_batch, output, T,
+                               _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img))
+        return video if n_samples is not None else video[0]
 
     @torch.no_grad()
     def animate(self, image, prompt: Union[str, torch.Tensor] = "", steps: int = 50, cfg_scale: float = 7.5,
                 eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                 timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
-                output: str = "uint8", video_length: Optional[int] = None) -> torch.Tensor:
+                output: str = "uint8", video_length: Optional[int] = None, n_samples: Optional[int] = None,
+                segments_per_batch: Optional[int] = None) -> torch.Tensor:
         """One image -> one T-frame video: image_guided_synthesis with interp=False, loop=False (inference.py:
         180-277; c_concat is the image's latent repeated over the T frames, :201-203), the image-to-video mode of
         the DynamiCrafter checkpoints.  image: a uint8 [H, W, 3] RGB image of any size; prompt: a string or token
         ids [1, 77].  The image's posterior noise comes from a CPU generator seeded `seed`, x_T and the DDIM step
         noise from a generator on the model's device seeded `seed` (keyframe 0 / segment 0 of `interpolate`); a
-        dual-reference first stage gets the image's encoder maps as both reference frames.  video_length: T, as for
-        interpolate.
+        dual-reference first stage gets the image's encoder maps as both reference frames.  video_length: T, and
+        n_samples / segments_per_batch (variants sampled per call), as for interpolate.
 
         Returns uint8 [T, size[0], size[1], 3] on the model's device; with output="float", the spliced video before
-        quantisation, float32 [3, T, size[0], size[1]]."""
+        quantisation, float32 [3, T, size[0], size[1]]; with an integer n_samples, [n, T, H, W, 3] / [n, 3, T, H, W]."""
         T = check_video_length(self.model.temporal_length if video_length is None else video_length)
+        n = 1 if n_samples is None else check_n_samples(n_samples)
+        if segments_per_batch is None:
+            segments_per_batch = default_segments_per_batch(size, T)
         frames = self._preprocess([image], size, output)
-        video = self._generate(frames, prompt, [0], [0], False, steps, cfg_scale, eta, fs, guidance_rescale,
-                               timestep_spacing, cfg_img, False, seed, size, 1, output, T)
-        return video[0] if output == "float" else video
+        video = self._generate(frames, prompt, [0], [0], False, False, seed, n, segments_per_batch, output, T,
+                               _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img))
+        if output == "float":
+            video = video[:, 0]
+        return video if n_samples is not None else video[0]
 
-    def _preprocess(self, images, size, output) -> torch.Tensor:
-        """Argument checks shared by interpolate and animate, then preprocess() onto the model's device."""
-        m = self.model
+    @torch.no_grad()
+    def interpolate_pairs(self, pairs, prompts: Union[str, Sequence[str], torch.Tensor] = "", n_samples: int = 1,
+                          steps: int = 50, cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10,
+                          guidance_rescale: float = 0.7, timestep_spacing: str = "uniform_trailing", cfg_img=None,
+                          seed: int = 123, size=(320, 512), pairs_per_batch: Optional[int] = None,
+                          output: str = "uint8", video_length: Optional[int] = None) -> torch.Tensor:
+        """P independent keyframe pairs -> n_samples T-frame clips each: the reference's --prompt_dir --interp run
+        (module docstring).  pairs: P pairs of uint8 RGB images (a sequence of (a, b), or a tensor [P, 2, H, W, 3]);
+        prompts: one string for every pair, a list of P strings, or token ids [P, 77].
+
+        Pair i is the call interpolate([a_i, b_i], prompts=p_i, seed=seed + i, n_samples=n, segments_per_batch=n):
+        bit for bit with pairs_per_batch=1, on any number of ranks; to the kernels' batch tiling with larger groups.
+        pairs_per_batch: pairs whose keyframes are encoded, conditioned and sampled together (pairs_per_batch x n rows
+        per sample() call); None: default_pairs_per_batch(size, T, n).
+
+        Returns uint8 [P, n, T, size[0], size[1], 3] on the model's device, every pair's whole clip; with
+        output="float", float32 [P, n, 3, T, size[0], size[1]]."""
+        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
+        n = check_n_samples(n_samples)
+        P = len(pairs)
+        if P < 1 or any(len(p) != 2 for p in pairs):
+            raise ValueError("pairs must be a non-empty sequence of (image, image) pairs")
+        if isinstance(prompts, torch.Tensor):
+            if prompts.dim() != 2 or prompts.shape[0] != P:
+                raise ValueError(f"token ids must be [P={P}, 77], got {tuple(prompts.shape)}")
+        elif not isinstance(prompts, str) and len(prompts) != P:
+            raise ValueError(f"{len(prompts)} prompts for {P} pairs")
+        if pairs_per_batch is None:
+            pairs_per_batch = default_pairs_per_batch(size, T, n)
+        elif isinstance(pairs_per_batch, bool) or not isinstance(pairs_per_batch, int) or pairs_per_batch < 1:
+            raise ValueError(f"pairs_per_batch must be an integer >= 1, got {pairs_per_batch!r}")
+        self._check_arguments(size, output)
+        sampling = _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img)
+        self._check_latency(sampling)
+        dev = self.model.device
+        video = (torch.empty(P * n * T, size[0], size[1], 3, dtype=torch.uint8, device=dev) if output == "uint8"
+                 else torch.empty(P * n, 3, T, size[0], size[1], dtype=torch.float32, device=dev))
+        mine = self._mine(P)
+        for g0 in range(0, len(mine), pairs_per_batch):
+            group = mine[g0:g0 + pairs_per_batch]
+            frames = preprocess([im for i in group for im in pairs[i]], size, dev)
+            text = prompts if isinstance(prompts, str) else (prompts[group] if isinstance(prompts, torch.Tensor)
+                                                             else [prompts[i] for i in group])
+            # pair-major rows: pair i's variant v is video row i * n + v, whole (frames 0 .. T-1, no seam)
+            rows = [(k, seed + i + v * VARIANT_SEED_STRIDE, i * n + v if output == "float" else (0, T, (i * n + v) * T))
+                    for k, i in enumerate(group) for v in range(n)]
+            G = len(group)
+            self._render(frames, text, [2 * k for k in range(G)], [2 * k + 1 for k in range(G)], True,
+                         [seed + i + j for i in group for j in (0, 1)], rows, len(rows), video, T, sampling)
+        per_pair = n if output == "float" else n * T
+        self._broadcast(video, P, lambda i0, i1: (i0 * per_pair, i1 * per_pair))
+        return (video.view(P, n, T, size[0], size[1], 3) if output == "uint8"
+                else video.view(P, n, 3, T, size[0], size[1]))
+
+    def _check_arguments(self, size, output) -> None:
         if output not in ("uint8", "float"):
             raise ValueError(f"output must be 'uint8' or 'float', got {output!r}")
         if size[0] % 16 or size[1] % 16:
             raise ValueError(f"size {tuple(size)} must be a multiple of 16")
-        if m.model.conditioning_key != "hybrid":
+        if self.model.model.conditioning_key != "hybrid":
             raise NotImplementedError("image-conditioned synthesis needs the hybrid (concat + cross-attention) model")
-        return preprocess(images, size, m.device)
 
-    def _generate(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
-                  timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, T) -> torch.Tensor:
-        """S = len(first) segments of T frames; segment k runs from keyframe first[k] to keyframe last[k] (interp), or animates
-        keyframe first[k] (not interp).  With a group, this rank computes its block of segments and the blocks are
-        then broadcast."""
-        if self.latency:
-            if cfg_img is not None:
-                raise NotImplementedError("latency mode splits two guidance branches over a GPU pair; three-way "
-                                          "guidance (cfg_img) is not supported")
-            if cfg_scale == 1.0:
-                raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
-                                 "cfg_scale 1.0 has no unconditional branch")
-        S = len(first)
-        F = (T - 1) * S + (0 if loop else 1)
-        video = (torch.empty(F, size[0], size[1], 3, dtype=torch.uint8, device=self.model.device) if output == "uint8"
-                 else torch.empty(S, 3, T, size[0], size[1], dtype=torch.float32, device=self.model.device))
-        mine = list(range(S)) if self.group is None else distributed.shard_clips(S, self._block, self._n_blocks)
-        if mine:
-            self._render(frames, prompts, first, last, interp, steps, cfg_scale, eta, fs, guidance_rescale,
-                         timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video, T)
+    def _preprocess(self, images, size, output) -> torch.Tensor:
+        """Argument checks shared by interpolate and animate, then preprocess() onto the model's device."""
+        self._check_arguments(size, output)
+        return preprocess(images, size, self.model.device)
+
+    def _check_latency(self, sampling) -> None:
+        if not self.latency:
+            return
+        if sampling["cfg_img"] is not None:
+            raise NotImplementedError("latency mode splits two guidance branches over a GPU pair; three-way "
+                                      "guidance (cfg_img) is not supported")
+        if sampling["cfg_scale"] == 1.0:
+            raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
+                             "cfg_scale 1.0 has no unconditional branch")
+
+    def _mine(self, n_items: int):
+        """The items (rows, pairs) of this rank's block: all of them without a group."""
+        return list(range(n_items)) if self.group is None else distributed.shard_clips(n_items, self._block,
+                                                                                       self._n_blocks)
+
+    def _broadcast(self, video, n_items: int, span) -> None:
+        """With a group: give every rank the whole `video`, block b's items [i0, i1) being video[span(i0, i1)] of
+        the rank that computed them."""
         if self.group is None:
-            return video
+            return
         blocks = []
         for b in range(self._n_blocks):
-            seg = distributed.shard_clips(S, b, self._n_blocks)
-            if not seg:
-                continue
-            k0, k1 = seg[0], seg[-1]
-            if output == "float":
-                blocks.append((self._owner(b), k0, k1 + 1))
-            else:                                                   # the frames tc_video_u8 writes for the block
-                blocks.append((self._owner(b), (T - 1) * k0 + (1 if k0 else 0),
-                               (T - 1) * k1 + (T - 1 if (loop and k1 == S - 1) else T)))
+            items = distributed.shard_clips(n_items, b, self._n_blocks)
+            if items:
+                blocks.append((self._owner(b),) + tuple(span(items[0], items[-1] + 1)))
         distributed.broadcast_blocks(video, blocks, self.group)
-        return video
 
-    def _render(self, frames, prompts, first, last, interp: bool, steps, cfg_scale, eta, fs, guidance_rescale,
-                timestep_spacing, cfg_img, loop, seed, size, segments_per_batch, output, mine, video, T) -> None:
-        """Sample and decode segments `mine` (of S = len(first)) into their places in `video`."""
+    def _generate(self, frames, prompts, first, last, interp: bool, loop, seed, n, rows_per_batch, output, T,
+                  sampling) -> torch.Tensor:
+        """n variants of S = len(first) segments of T frames; segment k runs from keyframe first[k] to keyframe
+        last[k] (interp), or animates keyframe first[k] (not interp).  Row r = v * S + k is variant v of segment k.
+        With a group, this rank computes its block of rows and the blocks are then broadcast.  Returns uint8
+        [n, F, H, W, 3] or float [n, S, 3, T, H, W]."""
+        self._check_latency(sampling)
+        S = len(first)
+        H, W = frames.shape[-2:]
+        F = (T - 1) * S + (0 if loop else 1)
+        dev = self.model.device
+        video = (torch.empty(n * F, H, W, 3, dtype=torch.uint8, device=dev) if output == "uint8"
+                 else torch.empty(n * S, 3, T, H, W, dtype=torch.float32, device=dev))
+
+        def window(r):
+            """(f_begin, f_end, out_frame): the frames of row r's segment kept by the seam rule, and where the first
+            of them goes in the flattened [n * F] video (variant v's video starts at frame v * F)."""
+            v, k = divmod(r, S)
+            f_begin, f_end = (1 if k else 0), (T - 1 if (loop and k == S - 1) else T)
+            return f_begin, f_end, v * F + (T - 1) * k + f_begin
+
+        def span(r0, r1):                       # rows r0 .. r1-1 write one contiguous range (variant-major order)
+            if output == "float":
+                return r0, r1
+            a, b = window(r0), window(r1 - 1)
+            return a[2], b[2] + b[1] - b[0]
+
+        rows = [(r % S, seed + r % S + (r // S) * VARIANT_SEED_STRIDE, r if output == "float" else window(r))
+                for r in self._mine(n * S)]
+        if rows:
+            self._render(frames, prompts, first, last, interp, [seed + j for j in range(frames.shape[0])], rows,
+                         rows_per_batch, video, T, sampling)
+        self._broadcast(video, n * S, span)
+        return video.view(n, F, H, W, 3) if output == "uint8" else video.view(n, S, 3, T, H, W)
+
+    def _render(self, frames, prompts, first, last, interp: bool, key_seeds, rows, rows_per_batch, video, T,
+                sampling) -> None:
+        """Sample and decode `rows` into their places in `video`.  rows: [(segment k of S = len(first), the seed of
+        its x_T and step noise, its place)], sampled `rows_per_batch` at a time; the place is the row's index in
+        float `video` [R, 3, T, H, W], or (f_begin, f_end, out_frame) of tc_video_u8 for uint8 `video`.
+        key_seeds[j]: the seed of keyframe j's posterior noise."""
         m = self.model
         dev = m.device
         n_dec = m.en_and_decode_n_samples_a_time or m.temporal_length                # decode_core's chunk
         ex = runtime.TEST_EXECUTOR
         K, S = frames.shape[0], len(first)
+        steps, cfg_scale, cfg_img = sampling["steps"], sampling["cfg_scale"], sampling["cfg_img"]
 
         # conditioning: text over the distinct prompts + "", image over each segment's first keyframe + the zero image
-        # (over all S segments whatever `mine` is: the towers' batch size stays that of the single-process call)
+        # (over all S segments whatever the rows are: the towers' batch size stays that of the single-process call,
+        # and the variants of a segment share its conditioning)
         cond_emb, empty_emb = self._text(prompts, S)
         if m.uncond_type == "empty_seq":
             uc_emb = empty_emb.expand_as(cond_emb)
@@ -283,10 +417,11 @@ class ToonCrafterPipeline:
         img_all = m.image_proj_model(m.embedder(img))
         img_emb, uc_img_emb = img_all[:S], img_all[S:].expand(S, -1, -1)
 
-        # first stage: the K distinct keyframes once; keyframe j's posterior noise from a CPU generator seeded seed + j
+        # first stage: the K distinct keyframes once; keyframe j's posterior noise from a CPU generator seeded
+        # key_seeds[j]
         post, hidden = m.first_stage_model.encode(frames, return_hidden_states=True)
-        noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(seed + j))
-                             for j in range(K)])
+        noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(s))
+                             for s in key_seeds])
         z = m.get_first_stage_encoding(post, noise=noise)                           # [K, 4, h, w]
         h, w = z.shape[-2:]
         if interp:
@@ -302,8 +437,9 @@ class ToonCrafterPipeline:
         dec = m.first_stage_model.decoder_engine() if decodes else None
         dual_ref = isinstance(m.first_stage_model.decoder, VideoDecoder)
         keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
-        for g0 in range(0, len(mine), segments_per_batch):
-            seg = mine[g0:g0 + segments_per_batch]
+        for g0 in range(0, len(rows), rows_per_batch):
+            batch = rows[g0:g0 + rows_per_batch]
+            seg = [k for k, _, _ in batch]
             b = len(seg)
             cc = [c_concat[seg]]
             cond = {"c_crossattn": [torch.cat([cond_emb[seg], img_emb[seg]], 1)], "c_concat": cc}
@@ -313,16 +449,16 @@ class ToonCrafterPipeline:
             if cfg_img is not None:
                 extra = dict(cfg_img=cfg_img, unconditional_conditioning_img_nonetext={
                     "c_crossattn": [torch.cat([uc_emb[seg], img_emb[seg]], 1)], "c_concat": cc})
-            gens = [torch.Generator(device=dev).manual_seed(seed + k) for k in seg]
+            gens = [torch.Generator(device=dev).manual_seed(s) for _, s, _ in batch]
             samples, _ = sampler.sample(S=steps, conditioning=cond, batch_size=b, shape=[z.shape[1], T, h, w],
                                         verbose=False, unconditional_guidance_scale=cfg_scale,
-                                        unconditional_conditioning=uc, eta=eta,
-                                        fs=torch.tensor([fs] * b, dtype=torch.long, device=dev),
-                                        timestep_spacing=timestep_spacing, guidance_rescale=guidance_rescale,
-                                        noise_generators=gens, **extra)
+                                        unconditional_conditioning=uc, eta=sampling["eta"],
+                                        fs=torch.tensor([sampling["fs"]] * b, dtype=torch.long, device=dev),
+                                        timestep_spacing=sampling["timestep_spacing"],
+                                        guidance_rescale=sampling["guidance_rescale"], noise_generators=gens, **extra)
             if not decodes:
                 continue
-            for i, k in enumerate(seg):
+            for i, (k, _, place) in enumerate(batch):
                 lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
                 if dual_ref:
                     ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
@@ -335,16 +471,20 @@ class ToonCrafterPipeline:
                     # no splice at all (tc_video_u8 with x14 = NULL).
                     y16 = _decode_chunks(dec, lat, n_dec, None, ex)
                     y14 = None if T >= 6 else y16[keep]
-                if output == "float":
+                if video.dtype == torch.float32:
                     v = y16.float()
                     if y14 is not None:
                         v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
-                    video[k] = v.permute(1, 0, 2, 3)
+                    video[place] = v.permute(1, 0, 2, 3)
                     continue
-                f_begin = 0 if k == 0 else 1
-                f_end = T - 1 if (loop and k == S - 1) else T
-                args, kw = (y16, y14, video), dict(f_begin=f_begin, f_end=f_end, out_frame=(T - 1) * k + f_begin)
+                f_begin, f_end, out_frame = place
+                args, kw = (y16, y14, video), dict(f_begin=f_begin, f_end=f_end, out_frame=out_frame)
                 if ex is not None:
                     ex(ops.video_u8, args, kw)
                 else:
                     ops.video_u8(*args, **kw)
+
+
+def _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img) -> dict:
+    return dict(steps=steps, cfg_scale=cfg_scale, eta=eta, fs=fs, guidance_rescale=guidance_rescale,
+                timestep_spacing=timestep_spacing, cfg_img=cfg_img)
