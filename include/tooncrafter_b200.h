@@ -241,6 +241,15 @@ int tc_ddim_step(const void* e_c, const void* e_uc, const float* x, const float*
 int tc_ddim_step3(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
                   float* x_prev, float* pred_x0, const float* coef, int B, long long n, double* ws, void* stream);
 
+/* Forward diffusion of a clean latent, in place on x (fp32 [B][n]); row b takes a = coef[2b], c = coef[2b+1]:
+ *   q = clean ? x0 : a*x0 + c*noise        (q_sample / stochastic_encode: ddpm3d.py:306-309, ddim.py:309-318)
+ *   x = mask ? q*m + (1 - m)*x : q         (the masked step blend of ddim.py:172-180)
+ * x0, noise, mask: fp32 [B][n] (noise and coef may be NULL with clean; mask NULL: x = q).  Each multiply and add is
+ * rounded on its own in that order (no contraction), so x equals torch's fp32 arithmetic bit for bit.  x may not
+ * alias x0, noise or mask.  coef is a device pointer (2B floats), so a captured graph can be replayed with new ones. */
+int tc_q_sample(float* x, const float* x0, const float* noise, const float* mask, const float* coef, int clean, int B,
+                long long n, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -44,6 +44,13 @@ N as above (the maximum over ranks): seconds per call and per clip:
 
     python scripts/bench_pipeline.py --pairs 8 --gpus 1
     torchrun --nproc-per-node 2 scripts/bench_pipeline.py --pairs 8 --gpus 2
+
+--refine S [S ...] measures ToonCrafterPipeline.refine on a synthetic 16-frame clip at --size: interpolate() of the
+clip's first and last frames (K = 2), refine() at each strength S (int(S * steps) DDIM steps plus the encode of the
+16 frames), and refine(0.5, keep=[0, 1, 14, 15]) (the masked fused sampler), alternating; seconds per call and the
+peak device memory of each arm (warm-up at DDIM-4, so that every strength runs a step):
+
+    python scripts/bench_pipeline.py --refine 0.25 0.5 1.0
 """
 from __future__ import annotations
 
@@ -238,6 +245,40 @@ def bench_n_samples(args, model, info, build_s):
     return 0
 
 
+def bench_refine(args, model, info, build_s):
+    """interpolate against refine at each strength of args.refine and one keep case (see the module docstring)."""
+    from tooncrafter_b200.pipeline import ToonCrafterPipeline
+    size = tuple(args.size)
+    pipe = ToonCrafterPipeline(model)
+    clip = (torch.rand(16, size[0], size[1], 3, generator=torch.Generator().manual_seed(0)) * 255).to(torch.uint8)
+    arms = {"interpolate": lambda st: pipe.interpolate(clip[[0, 15]], steps=st, seed=123, size=size)}
+    for strength in args.refine:
+        arms[f"refine_{strength:g}"] = lambda st, s_=strength: pipe.refine(clip, s_, steps=st, seed=123, size=size)
+    arms["refine_0.5_keep"] = lambda st: pipe.refine(clip, 0.5, keep=[0, 1, 14, 15], steps=st, seed=123, size=size)
+    for fn in arms.values():
+        fn(4)
+    times, peaks = {a: [] for a in arms}, {a: 0 for a in arms}
+    for _ in range(args.reps):
+        for name, fn in arms.items():
+            dt, pk = _timed(lambda: fn(args.ddim_steps))
+            times[name].append(dt)
+            peaks[name] = max(peaks[name], pk)
+    rows = []
+    for name in arms:
+        best = min(times[name])
+        row = dict(arm=name, sec_per_call=best, all_s=[round(x, 3) for x in times[name]],
+                   peak_gib=peaks[name] / 2 ** 30, gpu=info)
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    out = dict(metric="refine a 16-frame clip: seconds per call (%dx%d, DDIM-%d, CFG 7.5, eta 1, synthetic weights, "
+               "%s first stage)" % (size[0], size[1], args.ddim_steps, args.first_stage), gpu=info, reps=args.reps,
+               model_build_s=build_s, configs=rows,
+               note="sec_per_call = best of the timed reps, host clock around work ending in a device synchronise; "
+                    "peak_gib = torch.cuda.max_memory_allocated over a timed call (model and cached plans included)")
+    print(json.dumps(out), flush=True)
+    return 0
+
+
 def bench_sharded(args, model, info, build_s, group):
     """--gpus N: K = 5 interpolate (or animate) sharded over `group` (None: one GPU); see the module docstring."""
     import torch.distributed as dist
@@ -301,7 +342,12 @@ def main():
                          "--pairs, the variants per pair")
     ap.add_argument("--pairs", type=int, default=None, metavar="P",
                     help="measure interpolate_pairs on P synthetic pairs over --gpus N (default 1)")
+    ap.add_argument("--refine", type=float, nargs="+", default=None, metavar="S",
+                    help="measure refine of a 16-frame clip at each of these strengths, against interpolate "
+                         "(docstring)")
     args = ap.parse_args()
+    if args.refine is not None and any(not 0.0 < x <= 1.0 for x in args.refine):
+        ap.error("--refine strengths lie in (0, 1]")
     if args.pairs is not None and args.gpus is None:
         args.gpus = 1
     if args.video_length is not None:
@@ -348,6 +394,8 @@ def main():
         return bench_video_length(args, model, info, build_s)
     if args.n_samples is not None:
         return bench_n_samples(args, model, info, build_s)
+    if args.refine is not None:
+        return bench_refine(args, model, info, build_s)
     pipe = ToonCrafterPipeline(model)
     g = torch.Generator().manual_seed(0)
     results = []

@@ -415,6 +415,30 @@ __global__ void video_u8_kernel(const __half* __restrict__ x16, const __half* __
     }
 }
 
+// ------------------------------------------------------------------------------------------------ forward diffusion
+// Row b = blockIdx.y of x [B][n], in place, with a = coef[2b], c = coef[2b+1]:
+//   q = clean ? x0 : a*x0 + c*noise                  (q_sample / stochastic_encode, ddpm3d.py:306-309, ddim.py:309-318)
+//   x = mask ? q*m + (1 - m)*x : q                   (the masked step blend of ddim.py:172-180)
+// Every multiply and add rounded on its own, in torch's op order, so the result is torch's fp32 arithmetic bit for bit.
+__global__ void q_sample_kernel(float* x, const float* __restrict__ x0, const float* __restrict__ noise,
+                                const float* __restrict__ mask, const float* __restrict__ coef, int clean,
+                                long long n) {
+    tc::pdl_wait();
+    const int b = blockIdx.y;
+    const float a = clean ? 0.f : coef[2 * b], c = clean ? 0.f : coef[2 * b + 1];
+    const long long off = (long long)b * n;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+         i += (long long)gridDim.x * blockDim.x) {
+        const float q = clean ? x0[off + i] : __fadd_rn(__fmul_rn(a, x0[off + i]), __fmul_rn(c, noise[off + i]));
+        float r = q;
+        if (mask) {
+            const float m = mask[off + i];
+            r = __fadd_rn(__fmul_rn(q, m), __fmul_rn(__fsub_rn(1.0f, m), x[off + i]));
+        }
+        x[off + i] = r;
+    }
+}
+
 inline int grid_for(long long total, int threads, int max_blocks) {
     long long g = (total + threads - 1) / threads;
     if (g > max_blocks) g = max_blocks;
@@ -574,6 +598,17 @@ extern "C" int tc_video_u8(const void* x16, const void* x14, int T, int H, int W
                     f_end - f_begin, reinterpret_cast<uint8_t*>(out), vec);
     count_launch();
     TC_CHECK_LAUNCH("video_u8_kernel");
+    return TC_OK;
+}
+
+extern "C" int tc_q_sample(float* x, const float* x0, const float* noise, const float* mask, const float* coef,
+                           int clean, int B, long long n, void* stream_v) {
+    TC_CHECK_ARG(x && x0 && B > 0 && B <= 65535 && n > 0 && (clean || (noise && coef)), "tc_q_sample: bad arguments");
+    cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_v);
+    const int g = grid_for(n, 256, (4 * sm_count() + B - 1) / B);
+    tc_host::launch(q_sample_kernel, dim3(g, B), dim3(256), 0, stream, 1, x, x0, noise, mask, coef, clean ? 1 : 0, n);
+    count_launch();
+    TC_CHECK_LAUNCH("q_sample_kernel");
     return TC_OK;
 }
 

@@ -29,6 +29,14 @@ DIR/<name of image 2i>_sample{v}/ (ToonCrafterPipeline.interpolate_pairs, pair i
     python -m tooncrafter_b200.interpolate --config ... --ckpt ... --prompt-dir prompts/512_interp --n-samples 4 \
         --out results/
 
+--init-video SRC instead refines an existing clip (ToonCrafterPipeline.refine): SRC is a directory of frame images, a
+uint8 [T, H, W, 3] .npy (what this command writes) or a video file OpenCV can read.  --strength S (required) re-runs
+int(S * steps) DDIM steps from the clip's latents; --keep-frames 0-3,12-15 holds those frames to the clip and
+regenerates the ones between:
+
+    python -m tooncrafter_b200.interpolate --config ... --ckpt ... --init-video out/video.npy --strength 0.5 \
+        --keep-frames 0-1,14-15 --out results/refined
+
 The config is the reference-style YAML (read with PyYAML; only its `model:` section is used, so the training
 configs, whose first stage is the plain AutoencoderKL, work as well).  Its two OpenCLIP conditioning targets
 (lvdm.modules.encoders.condition.FrozenOpenCLIP*) are pointed at this repository's classes unless
@@ -39,6 +47,7 @@ from __future__ import annotations
 import argparse
 import glob
 import os
+import re
 import sys
 
 import numpy as np
@@ -58,10 +67,18 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--synthetic-weights", action="store_true", help="seeded synthetic weights instead of --ckpt")
     ap.add_argument("--keep-config-targets", action="store_true",
                     help="keep the YAML's OpenCLIP targets instead of this repository's classes")
-    src = ap.add_mutually_exclusive_group(required=True)
+    src = ap.add_mutually_exclusive_group()        # one of them is required: main() checks
     src.add_argument("--frames", nargs="+", help="K >= 2 keyframe images, in order; one image: animate it")
     src.add_argument("--prompt-dir", default=None,
                      help="a directory of keyframe pairs and a prompt file, laid out as the reference's --prompt_dir")
+    src.add_argument("--init-video", default=None,
+                     help="refine this clip (ToonCrafterPipeline.refine): a directory of frame images, a uint8 "
+                          "[T, H, W, 3] .npy, or a video file OpenCV can read")
+    ap.add_argument("--strength", type=float, default=None,
+                    help="with --init-video (required there): share of the DDIM steps re-run, in (0, 1]")
+    ap.add_argument("--keep-frames", default=None,
+                    help="with --init-video: frames held to the clip, e.g. 0-3,12-15 (the frames between are "
+                         "regenerated)")
     ap.add_argument("--text-input", action="store_true",
                     help="with --prompt-dir: pair i gets line i of the prompt file (default: every pair gets \"\")")
     ap.add_argument("--n-samples", type=int, default=None,
@@ -168,6 +185,61 @@ def read_prompt_dir(data_dir: str, text_input: bool = False):
     return pairs, (lines if text_input else [""] * P), names
 
 
+def read_init_video(path: str) -> np.ndarray:
+    """The clip of --init-video as uint8 [T, H, W, 3] RGB: a directory of images (sorted as get_filelist sorts them,
+    what write_video writes as frame_%04d.png), a .npy array (write_video's video.npy), or any other file through
+    OpenCV's VideoCapture.  ValueError for a missing or unreadable source, or frames of different sizes."""
+    if os.path.isdir(path):
+        from PIL import Image
+        files = _filelist(path, IMAGE_SUFFIXES)
+        if not files:
+            raise ValueError(f"{path}: no images (*.{'|'.join(IMAGE_SUFFIXES)})")
+        frames = [np.asarray(Image.open(f).convert("RGB")) for f in files]
+        if len({f.shape for f in frames}) != 1:
+            raise ValueError(f"{path}: the images differ in size")
+        return np.stack(frames)
+    if not os.path.isfile(path):
+        raise ValueError(f"{path}: no such file or directory")
+    if path.endswith(".npy"):
+        v = np.load(path)
+        if v.dtype != np.uint8 or v.ndim != 4 or v.shape[-1] != 3:
+            raise ValueError(f"{path}: expected a uint8 [T, H, W, 3] array, got {v.dtype} {v.shape}")
+        return v
+    try:
+        import cv2
+    except ImportError:
+        raise ValueError(f"{path}: reading a video file needs OpenCV (cv2)") from None
+    cap = cv2.VideoCapture(path)
+    frames = []
+    while cap.isOpened():
+        ok, fr = cap.read()
+        if not ok:
+            break
+        frames.append(np.ascontiguousarray(fr[..., ::-1]))
+    cap.release()
+    if not frames:
+        raise ValueError(f"{path}: OpenCV read no frames")
+    return np.stack(frames)
+
+
+def parse_frame_ranges(spec: str, T: int) -> list:
+    """--keep-frames: comma-separated frame indices and inclusive ranges a-b ("0-3,12-15"), each within 0 .. T-1 and
+    listed once.  ValueError otherwise."""
+    out = []
+    for part in spec.split(","):
+        part = part.strip()
+        if not re.fullmatch(r"\d+(-\d+)?", part):
+            raise ValueError(f"--keep-frames: {part!r} is not a frame index or a range a-b")
+        a, _, b = part.partition("-")
+        lo, hi = int(a), int(b or a)
+        if not 0 <= lo <= hi < T:
+            raise ValueError(f"--keep-frames: {part!r} is not within frames 0 .. {T - 1}")
+        out.extend(range(lo, hi + 1))
+    if len(set(out)) != len(out):
+        raise ValueError(f"--keep-frames: {spec!r} lists a frame twice")
+    return out
+
+
 def read_prompts(args, n_segments: int):
     if args.prompts_file is None:
         return args.prompt
@@ -203,6 +275,8 @@ def write_video(video: np.ndarray, out_dir: str, fps: int) -> None:
 def main(argv=None) -> int:
     ap = get_parser()
     args = ap.parse_args(argv)
+    if args.frames is None and args.prompt_dir is None and args.init_video is None:
+        ap.error("one of the arguments --frames --prompt-dir is required (or --init-video to refine a clip)")
     from .pipeline import check_n_samples, check_video_length
     try:
         if args.video_length is not None:
@@ -224,6 +298,26 @@ def main(argv=None) -> int:
             ap.error(str(e))
     elif args.text_input or args.pairs_per_batch is not None:
         ap.error("--text-input and --pairs-per-batch apply to --prompt-dir")
+    args.clip = args.keep = None
+    if args.init_video is not None:
+        if args.strength is None:
+            ap.error("--init-video needs --strength")
+        if args.loop:
+            ap.error("--loop does not apply to --init-video")
+        try:
+            args.clip = read_init_video(args.init_video)
+            T = check_video_length(len(args.clip))
+            if args.video_length is not None and args.video_length != T:
+                raise ValueError(f"--video-length {args.video_length}: the clip has {T} frames")
+            if not 0.0 < args.strength <= 1.0 or int(args.strength * args.ddim_steps) < 1:
+                raise ValueError(f"--strength {args.strength} x --ddim-steps {args.ddim_steps} runs no DDIM step; "
+                                 "give a strength in (0, 1]")
+            if args.keep_frames is not None:
+                args.keep = parse_frame_ranges(args.keep_frames, T)
+        except ValueError as e:
+            ap.error(str(e))
+    elif args.strength is not None or args.keep_frames is not None:
+        ap.error("--strength and --keep-frames apply to --init-video")
     if not args.synthetic_weights and args.ckpt is None:
         raise SystemExit("give --ckpt, or --synthetic-weights for a run without a checkpoint")
     cfg = load_model_config(args.config, args.keep_config_targets)
@@ -264,13 +358,19 @@ def run(args, cfg, dev, group) -> int:
     writes = group is None or torch.distributed.get_rank() == 0
     if args.prompt_dir is not None:
         return run_prompt_dir(args, pipe, common, group, writes)
-    frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
-    if len(frames) == 1:
+    if args.clip is not None:
+        common.pop("video_length")
+        video = pipe.refine(args.clip, args.strength, prompt=read_prompts(args, 1), keep=args.keep, seed=args.seed,
+                            n_samples=args.n_samples, segments_per_batch=args.segments_per_batch, **common)
+        frames = args.clip
+    elif len(args.frames) == 1:
+        frames = [np.asarray(Image.open(args.frames[0]).convert("RGB"))]
         if args.loop:
             raise SystemExit("--loop needs at least two keyframes")
         video = pipe.animate(frames[0], prompt=read_prompts(args, 1), seed=args.seed, n_samples=args.n_samples,
                              **common)
     else:
+        frames = [np.asarray(Image.open(p).convert("RGB")) for p in args.frames]
         n_seg = len(frames) if args.loop else len(frames) - 1
         video = pipe.interpolate(frames, prompts=read_prompts(args, n_seg), loop=args.loop, seed=args.seed,
                                  segments_per_batch=args.segments_per_batch, n_samples=args.n_samples, **common)
@@ -282,7 +382,8 @@ def run(args, cfg, dev, group) -> int:
     else:
         for i, variant in enumerate(v):
             write_video(variant, os.path.join(args.out, f"sample{i}"), args.fps)
-    print(f"{len(frames)} {'image' if len(frames) == 1 else 'keyframes'} -> "
+    what = "frames refined" if args.clip is not None else ("image" if len(frames) == 1 else "keyframes")
+    print(f"{len(frames)} {what} -> "
           f"{'' if args.n_samples is None else f'{v.shape[0]} x '}{v.shape[-4]} frames of {v.shape[-3]}x{v.shape[-2]} "
           f"in {args.out}")
     return 0

@@ -339,5 +339,21 @@ def ddim_step3(e_c, e_uc, e_img, x, noise, x_prev, pred_x0, coef, ws, *, B: int,
           "tc_ddim_step3")
 
 
+def q_sample(x, x0, noise, mask, coef, *, B: int, n: int, clean: bool = False) -> None:
+    """In place on x (fp32 [B][n]): q = x0 if clean else coef[2b]*x0 + coef[2b+1]*noise per row b, then x = q where
+    mask is None, else q*mask + (1 - mask)*x.  torch's fp32 op order, bit for bit.  x0 / noise / mask: contiguous fp32
+    [B][n] (noise may be None with clean); coef: device fp32 [2B] (may be None with clean)."""
+    for name, t in (("x", x), ("x0", x0), ("noise", noise), ("mask", mask)):
+        if t is None:
+            continue
+        if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or t.numel() != B * n:
+            raise ValueError(f"q_sample: {name} must be a contiguous CUDA float32 tensor of {B} x {n} elements")
+    if coef is not None and (coef.dtype != torch.float32 or not coef.is_cuda or coef.numel() < 2 * B):
+        raise ValueError(f"q_sample: coef must be a CUDA float32 tensor of at least {2 * B} elements")
+    lib = _lib.load()
+    check(lib.tc_q_sample(x.data_ptr(), x0.data_ptr(), _ptr(noise), _ptr(mask), _ptr(coef), 1 if clean else 0, B, n,
+                          _stream()), "tc_q_sample")
+
+
 def launch_count() -> int:
     return int(_lib.load().tc_launch_count())

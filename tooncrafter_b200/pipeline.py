@@ -73,7 +73,7 @@ import torch.distributed as dist
 
 from . import distributed, ops, runtime
 from .modules import VideoDecoder, clip_tokenize
-from .sampler import DDIMSampler, DDIMSamplerMultiCond
+from .sampler import DDIMSampler, DDIMSamplerMultiCond, randn_rows
 
 
 def preprocess(keyframes, size=(320, 512), device="cpu") -> torch.Tensor:
@@ -262,6 +262,59 @@ class ToonCrafterPipeline:
         return video if n_samples is not None else video[0]
 
     @torch.no_grad()
+    def refine(self, clip, strength: float, prompt: Union[str, torch.Tensor] = "", keep: Optional[Sequence[int]] = None,
+               steps: int = 50, cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
+               timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
+               output: str = "uint8", n_samples: Optional[int] = None,
+               segments_per_batch: Optional[int] = None) -> torch.Tensor:
+        """Re-render an existing clip (SDEdit: DDIMSampler.stochastic_encode, then the last k DDIM steps), conditioned
+        on its own first and last frames exactly as interpolate([clip[0], clip[T-1]], video_length=T) is.
+
+        clip: T uint8 RGB frames (tensor [T, H, W, 3], ndarray, or a list of [H, W, 3] arrays), T even from 4 to 64.
+        strength in (0, 1]: k = int(strength * steps) >= 1 DDIM steps run, from the clip's latents noised to DDIM
+        index k - 1 (the noise level of the first step that runs); strength 1.0 is full sampling.  keep: None, or
+        frame indices whose latents are held to the clip's (the sampler's mask / x0: at every step those frames are
+        replaced by the clip's latents noised to the step's level), so only the frames between are regenerated.
+        Kept frames are decoded again with the rest, not pasted back, so they are close to, not equal to, the input.
+
+        First stage: frames 0 and T-1 are encoded as interpolate encodes its two keyframes (one N = 2 call, posterior
+        noise seeds `seed` and `seed + 1`), frames 1 .. T-2 in chunks of en_and_decode_n_samples_a_time (default
+        temporal_length) frames, frame j with posterior noise seed `seed + 1 + j`.  Variant v draws, from its device
+        generator seeded seed + v * VARIANT_SEED_STRIDE, first the encode noise (where interpolate draws x_T), then each
+        step's q_sample noise of the kept frames (with keep) and DDIM noise.  Under a zero-terminal-SNR schedule
+        (sqrt(alphas_cumprod[999]) = 0) refine(clip, 1.0) is therefore interpolate([clip[0], clip[-1]],
+        video_length=T) bit for bit.
+
+        Returns what a one-segment interpolate returns: uint8 [T, size[0], size[1], 3], or float32 [3, T, size[0],
+        size[1]] with output="float"; an integer n_samples adds a leading variant axis.  ValueError for a bad clip
+        length, strength, keep, n_samples or output before any work."""
+        T = check_video_length(len(clip))
+        if (isinstance(strength, bool) or not isinstance(strength, (int, float, np.integer, np.floating))
+                or not 0.0 < strength <= 1.0):
+            raise ValueError(f"strength must be a number in (0, 1], got {strength!r}")
+        k = int(strength * steps)
+        if k < 1:
+            raise ValueError(f"strength {strength} x steps {steps} runs no DDIM step (int(strength * steps) < 1)")
+        if keep is not None:
+            keep = list(keep)
+            if any(isinstance(j, bool) or not isinstance(j, (int, np.integer)) or not 0 <= j < T for j in keep):
+                raise ValueError(f"keep must hold frame indices from 0 to {T - 1}, got {keep!r}")
+            if len(set(int(j) for j in keep)) != len(keep):
+                raise ValueError(f"keep lists a frame twice: {keep!r}")
+            keep = sorted(int(j) for j in keep) or None
+        n = 1 if n_samples is None else check_n_samples(n_samples)
+        if segments_per_batch is None:
+            segments_per_batch = default_segments_per_batch(size, T)
+        frames = self._preprocess(clip, size, output)
+        init = dict(frames=frames[1:T - 1], seeds=[seed + 1 + j for j in range(1, T - 1)], k=k, keep=keep)
+        video = self._generate(frames[[0, T - 1]], prompt, [0], [1], True, False, seed, n, segments_per_batch, output,
+                               T, _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img),
+                               init=init)
+        if output == "float":
+            video = video[:, 0]
+        return video if n_samples is not None else video[0]
+
+    @torch.no_grad()
     def interpolate_pairs(self, pairs, prompts: Union[str, Sequence[str], torch.Tensor] = "", n_samples: int = 1,
                           steps: int = 50, cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10,
                           guidance_rescale: float = 0.7, timestep_spacing: str = "uniform_trailing", cfg_img=None,
@@ -356,11 +409,11 @@ class ToonCrafterPipeline:
         distributed.broadcast_blocks(video, blocks, self.group)
 
     def _generate(self, frames, prompts, first, last, interp: bool, loop, seed, n, rows_per_batch, output, T,
-                  sampling) -> torch.Tensor:
+                  sampling, init=None) -> torch.Tensor:
         """n variants of S = len(first) segments of T frames; segment k runs from keyframe first[k] to keyframe
         last[k] (interp), or animates keyframe first[k] (not interp).  Row r = v * S + k is variant v of segment k.
-        With a group, this rank computes its block of rows and the blocks are then broadcast.  Returns uint8
-        [n, F, H, W, 3] or float [n, S, 3, T, H, W]."""
+        With a group, this rank computes its block of rows and the blocks are then broadcast.  init: see _render.
+        Returns uint8 [n, F, H, W, 3] or float [n, S, 3, T, H, W]."""
         self._check_latency(sampling)
         S = len(first)
         H, W = frames.shape[-2:]
@@ -386,16 +439,21 @@ class ToonCrafterPipeline:
                 for r in self._mine(n * S)]
         if rows:
             self._render(frames, prompts, first, last, interp, [seed + j for j in range(frames.shape[0])], rows,
-                         rows_per_batch, video, T, sampling)
+                         rows_per_batch, video, T, sampling, init)
         self._broadcast(video, n * S, span)
         return video.view(n, F, H, W, 3) if output == "uint8" else video.view(n, S, 3, T, H, W)
 
     def _render(self, frames, prompts, first, last, interp: bool, key_seeds, rows, rows_per_batch, video, T,
-                sampling) -> None:
+                sampling, init=None) -> None:
         """Sample and decode `rows` into their places in `video`.  rows: [(segment k of S = len(first), the seed of
         its x_T and step noise, its place)], sampled `rows_per_batch` at a time; the place is the row's index in
         float `video` [R, 3, T, H, W], or (f_begin, f_end, out_frame) of tc_video_u8 for uint8 `video`.
-        key_seeds[j]: the seed of keyframe j's posterior noise."""
+        key_seeds[j]: the seed of keyframe j's posterior noise.
+
+        init (refine; one segment whose keyframes 0 and 1 are the clip's first and last frames): dict(frames=the
+        preprocessed frames 1 .. T-2, seeds=their posterior-noise seeds, k=DDIM steps to run, keep=None or kept frame
+        indices).  Every row then starts from the clip's latents stochastic_encode'd to DDIM index k - 1 with noise
+        drawn first from the row's generator, and samples the last k steps (with keep: mask / x0 on those frames)."""
         m = self.model
         dev = m.device
         n_dec = m.en_and_decode_n_samples_a_time or m.temporal_length                # decode_core's chunk
@@ -430,6 +488,12 @@ class ToonCrafterPipeline:
             c_concat[:, :, -1] = z[last]
         else:
             c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
+        if init is not None:
+            x0 = self._clip_latents(z, init["frames"], init["seeds"])                  # [1, 4, T, h, w]
+            mask = None
+            if init["keep"] is not None:
+                mask = torch.zeros(1, 1, T, 1, 1, dtype=torch.float32, device=dev)
+                mask[:, :, init["keep"]] = 1.0
 
         sampler = DDIMSampler(m) if cfg_img is None else DDIMSamplerMultiCond(m)
         sampler.latency_group = self._pair
@@ -450,6 +514,14 @@ class ToonCrafterPipeline:
                 extra = dict(cfg_img=cfg_img, unconditional_conditioning_img_nonetext={
                     "c_crossattn": [torch.cat([uc_emb[seg], img_emb[seg]], 1)], "c_concat": cc})
             gens = [torch.Generator(device=dev).manual_seed(s) for _, s, _ in batch]
+            if init is not None:
+                shape = (b, z.shape[1], T, h, w)
+                sampler.make_schedule(steps, sampling["timestep_spacing"], sampling["eta"], verbose=False)
+                x_k = sampler.stochastic_encode(x0.expand(shape), torch.full((b,), init["k"] - 1, device=dev),
+                                                noise=randn_rows(shape, dev, gens))
+                extra = dict(extra, x_T=x_k, t_start=init["k"])
+                if mask is not None:
+                    extra.update(mask=mask, x0=x0.expand(shape).contiguous())
             samples, _ = sampler.sample(S=steps, conditioning=cond, batch_size=b, shape=[z.shape[1], T, h, w],
                                         verbose=False, unconditional_guidance_scale=cfg_scale,
                                         unconditional_conditioning=uc, eta=sampling["eta"],
@@ -483,6 +555,22 @@ class ToonCrafterPipeline:
                     ex(ops.video_u8, args, kw)
                 else:
                     ops.video_u8(*args, **kw)
+
+    def _clip_latents(self, z_ends, interior, seeds) -> torch.Tensor:
+        """[1, 4, T, h, w] latents of a clip: frames 0 and T-1 from z_ends [2, 4, h, w], frames 1 .. T-2 encoded from
+        `interior` in chunks of decode_core's chunk length (the encoder is per frame, so chunking changes only its
+        batch tiling), frame j's posterior noise from a CPU generator seeded seeds[j - 1]."""
+        m = self.model
+        n_enc = m.en_and_decode_n_samples_a_time or m.temporal_length
+        T = interior.shape[0] + 2
+        x0 = torch.empty((1, z_ends.shape[1], T) + tuple(z_ends.shape[-2:]), dtype=z_ends.dtype, device=z_ends.device)
+        x0[0, :, 0], x0[0, :, T - 1] = z_ends[0], z_ends[1]
+        for i in range(0, T - 2, n_enc):
+            post = m.first_stage_model.encode(interior[i:i + n_enc])
+            noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(s))
+                                 for s in seeds[i:i + n_enc]])
+            x0[0, :, 1 + i:1 + i + post.mean.shape[0]] = m.get_first_stage_encoding(post, noise=noise).transpose(0, 1)
+        return x0
 
 
 def _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img) -> dict:

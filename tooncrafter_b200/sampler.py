@@ -1,10 +1,11 @@
 """DDIMSampler with the reference's public API (lvdm/models/samplers/ddim.py:10-279), H100-native inside.
 
 Fast path (the configuration scripts/run.sh uses: v-parameterisation, classifier-free guidance with a conditioning
-dict, no mask / corrector / quantiser): per step ONE batched UNet program replay (cond and uncond rows as B = 2b,
-CUDA graph) + ONE fused DDIM-update launch pair (tc_ddim_step: CFG combine in fp16 like ddim.py:226, per-sample
-std reductions, guidance rescale, v -> eps / x0, dynamic rescale, x_prev) with the step coefficients taken from a
-device table — no per-step `.item()` synchronisation, no materialised torch.full tensors.
+dict, no corrector / quantiser, with or without mask / x0): per step ONE batched UNet program replay (cond and uncond
+rows as B = 2b, CUDA graph) + ONE fused DDIM-update launch pair (tc_ddim_step: CFG combine in fp16 like ddim.py:226,
+per-sample std reductions, guidance rescale, v -> eps / x0, dynamic rescale, x_prev) with the step coefficients taken
+from a device table — no per-step `.item()` synchronisation, no materialised torch.full tensors.  With a mask, one
+tc_q_sample launch per step blends the noised x0 in before the replay (ddim.py:172-180).
 
 Any other option combination falls back to the general path below, which follows the reference control flow with
 torch elementwise plumbing around `model.apply_model` (still the CUDA UNet engine).
@@ -111,10 +112,22 @@ class DDIMSampler(object):
                noise_dropout=0.0, score_corrector=None, corrector_kwargs=None, verbose=True, schedule_verbose=False,
                x_T=None, log_every_t=100, unconditional_guidance_scale=1.0, unconditional_conditioning=None,
                precision=None, fs=None, timestep_spacing="uniform", guidance_rescale=0.0, **kwargs):
-        """Reference signature, plus `noise_generators`: None (the global RNG, as the reference) or one torch.Generator
-        per batch row on the model's device, from which that row's x_T (when not given) and every step's DDIM noise
-        are drawn."""
+        """Reference signature, plus two keywords of this library:
+
+        noise_generators: None (the global RNG, as the reference) or one torch.Generator per batch row on the model's
+        device, from which that row's x_T (when not given) and every step's DDIM noise are drawn; with `mask` (and
+        not clean_cond) also each step's q_sample noise of x0, drawn before that step's DDIM noise.
+
+        t_start: None, or k in 1 .. S: run only the last k DDIM steps (indices k-1 .. 0) from `x_T`, which is then
+        required (the SDEdit pair with stochastic_encode at DDIM index k-1; `decode` is this for the reference)."""
         noise_generators = kwargs.pop("noise_generators", None)
+        t_start = kwargs.pop("t_start", None)
+        if t_start is not None:
+            if isinstance(t_start, bool) or not isinstance(t_start, (int, np.integer)) or not 1 <= t_start <= S:
+                raise ValueError(f"t_start must be an integer from 1 to S={S}, got {t_start!r}")
+            if x_T is None:
+                raise ValueError("t_start needs x_T: the latent to continue from")
+            kwargs["t_start"] = int(t_start)
         if conditioning is not None:
             first = conditioning[list(conditioning.keys())[0]] if isinstance(conditioning, dict) else conditioning
             cbs = (first[0] if isinstance(first, (list, tuple)) else first).shape[0]
@@ -131,12 +144,49 @@ class DDIMSampler(object):
                                   precision=precision, fs=fs, guidance_rescale=guidance_rescale,
                                   noise_generators=noise_generators, **kwargs)
 
+    @torch.no_grad()
+    def stochastic_encode(self, x0, t, use_original_steps=False, noise=None):
+        """ddim.py:303-318: x0 noised to the level of per-row index t, a long tensor [B] of DDIM indices (of the last
+        make_schedule), or of DDPM timesteps with use_original_steps.  noise None: torch.randn_like(x0).  A CUDA fp32
+        x0 goes through tc_q_sample (the same fp32 arithmetic, bit for bit)."""
+        if use_original_steps:
+            sqrt_ac, sqrt_1mac = self.sqrt_alphas_cumprod, self.sqrt_one_minus_alphas_cumprod
+        else:
+            sqrt_ac, sqrt_1mac = torch.sqrt(self.ddim_alphas), self.ddim_sqrt_one_minus_alphas
+        if noise is None:
+            noise = torch.randn_like(x0)
+        t = torch.as_tensor(t, device=sqrt_ac.device)
+        if not (x0.is_cuda and x0.dtype == torch.float32 and noise.dtype == torch.float32):
+            size = (t.shape[0],) + (1,) * (x0.dim() - 1)
+            return sqrt_ac.gather(-1, t).reshape(size) * x0 + sqrt_1mac.gather(-1, t).reshape(size) * noise
+        B = x0.shape[0]
+        if t.shape != (B,):
+            raise ValueError(f"stochastic_encode: t must hold one index per row, [{B}], got {tuple(t.shape)}")
+        coef = torch.stack([sqrt_ac.gather(-1, t), sqrt_1mac.gather(-1, t)], 1).to(x0.device, torch.float32)
+        x0c = x0.contiguous()
+        out = torch.empty_like(x0c)
+        ops.q_sample(out, x0c, noise.expand(x0.shape).contiguous(), None, coef.reshape(-1), B=B, n=x0c[0].numel())
+        return out
+
+    @torch.no_grad()
+    def decode(self, x_latent, cond, t_start, unconditional_guidance_scale=1.0, unconditional_conditioning=None,
+               use_original_steps=False, callback=None):
+        """ddim.py:282-300: the last t_start steps of the last make_schedule's DDIM schedule (of the DDPM schedule with
+        use_original_steps) from x_latent, without fs (the model's default_fs) or guidance rescale.  Runs on the fused
+        path under the same conditions as sample()."""
+        img, _ = self.ddim_sampling(cond, tuple(x_latent.shape), x_T=x_latent,
+                                    ddim_use_original_steps=use_original_steps, callback=callback,
+                                    unconditional_guidance_scale=unconditional_guidance_scale,
+                                    unconditional_conditioning=unconditional_conditioning, verbose=False,
+                                    t_start=t_start)
+        return img
+
     def _fast_path_ok(self, cond, uc, cfg_scale, mask, quantize, corrector, noise_dropout, precision, orig_steps,
                       shape, kwargs=None):
         m = self.model
         unet = getattr(getattr(m, "model", None), "diffusion_model", None)
         return (m.parameterization == "v" and uc is not None and cfg_scale != 1.0 and isinstance(cond, dict)
-                and isinstance(uc, dict) and mask is None and not quantize and corrector is None
+                and isinstance(uc, dict) and not quantize and corrector is None
                 and noise_dropout == 0.0 and precision is None and not orig_steps and len(shape) == 5
                 and getattr(m.model, "conditioning_key", None) == "hybrid" and hasattr(unet, "layout")
                 and (m.device.type == "cuda" or getattr(self, "_test_executor", None) is not None))
@@ -146,7 +196,7 @@ class DDIMSampler(object):
                       quantize_denoised=False, mask=None, x0=None, img_callback=None, log_every_t=100,
                       temperature=1.0, noise_dropout=0.0, score_corrector=None, corrector_kwargs=None,
                       unconditional_guidance_scale=1.0, unconditional_conditioning=None, verbose=True,
-                      precision=None, fs=None, guidance_rescale=0.0, noise_generators=None, **kwargs):
+                      precision=None, fs=None, guidance_rescale=0.0, noise_generators=None, t_start=None, **kwargs):
         device = self.model.betas.device
         b = shape[0]
         img = randn_rows(shape, device, noise_generators) if x_T is None else x_T
@@ -157,6 +207,8 @@ class DDIMSampler(object):
         elif not ddim_use_original_steps:
             subset_end = int(min(timesteps / self.ddim_timesteps.shape[0], 1) * self.ddim_timesteps.shape[0]) - 1
             timesteps = self.ddim_timesteps[:subset_end]
+        if t_start is not None:                          # the last t_start steps only (ddim.py:284-287)
+            timesteps = min(timesteps, t_start) if ddim_use_original_steps else timesteps[:t_start]
         intermediates = {"x_inter": [img], "pred_x0": [img]}
         time_range = reversed(range(0, timesteps)) if ddim_use_original_steps else np.flip(timesteps)
         total_steps = timesteps if ddim_use_original_steps else timesteps.shape[0]
@@ -169,14 +221,18 @@ class DDIMSampler(object):
                                       list(time_range), total_steps, unconditional_guidance_scale, guidance_rescale,
                                       temperature, fs, callback, img_callback, log_every_t, intermediates,
                                       cfg_img=self._cfg_img(unconditional_guidance_scale, kwargs),
-                                      noise_generators=noise_generators)
+                                      noise_generators=noise_generators, mask=mask, x0=x0, clean_cond=clean_cond)
 
         for i, step in enumerate(time_range):
             index = total_steps - i - 1
             ts = torch.full((b,), int(step), device=device, dtype=torch.long)
             if mask is not None:
                 assert x0 is not None
-                img_orig = x0 if clean_cond else self.model.q_sample(x0, ts)
+                if clean_cond:
+                    img_orig = x0
+                else:
+                    q_noise = None if noise_generators is None else randn_rows(x0.shape, device, noise_generators)
+                    img_orig = self.model.q_sample(x0, ts, noise=q_noise)
                 img = img_orig * mask + (1.0 - mask) * img
             img, pred_x0 = self.p_sample_ddim(img, cond, ts, index=index, use_original_steps=ddim_use_original_steps,
                                               quantize_denoised=quantize_denoised, temperature=temperature,
@@ -217,11 +273,14 @@ class DDIMSampler(object):
                 float(self.model.sqrt_one_minus_alphas_cumprod[t]), rescale, float(a_prev.sqrt()),
                 float((1.0 - a_prev - sigma ** 2).sqrt()), float(sigma) * float(temperature)]
 
-    def _fused_setup(self, cond, uc, shape, steps, cfg_scale, phi, temperature, fs, extra_branches=(), cfg_img=None):
+    def _fused_setup(self, cond, uc, shape, steps, cfg_scale, phi, temperature, fs, extra_branches=(), cfg_img=None,
+                     q_coefficients=False):
         """Everything of the fused path that is per-`sample()` call: engine / plan lookup, conditioning K/V program,
         concat channels, fps, and the device tables of per-step coefficients.  `steps` = [(ddim index, t), ...] in
         execution order.  `extra_branches`: further conditioning dicts batched after [cond, uncond] (the multi-condition
-        sampler's image-without-text branch, with `cfg_img`).  Returns the state `_fused_step` consumes."""
+        sampler's image-without-text branch, with `cfg_img`).  q_coefficients: each table row also holds, from column
+        st.q_off, tc_q_sample's per-row pair (sqrt_alphas_cumprod[t], sqrt_one_minus_alphas_cumprod[t]) for the b rows
+        (the masked blend of ddpm3d.py:306-309).  Returns the state `_fused_step` consumes."""
         from .engine import _P
         m = self.model
         dev = m.device
@@ -258,8 +317,11 @@ class DDIMSampler(object):
         if len(extra_branches) > 1 or (extra_branches and group is not None):
             raise NotImplementedError("fused path: at most one extra guidance branch, not in latency mode")
         tail = [float(cfg_img)] if st.three else []
-        st.coef_table = torch.tensor([self.step_coefficients(index, cfg_scale, phi, temperature) + tail
-                                      for index, _ in steps], dtype=torch.float32, device=dev)
+        st.q_off = 8 + len(tail)
+        q = lambda t: ([float(m.sqrt_alphas_cumprod[t]), float(m.sqrt_one_minus_alphas_cumprod[t])] * b
+                       if q_coefficients else [])
+        st.coef_table = torch.tensor([self.step_coefficients(index, cfg_scale, phi, temperature) + tail + q(int(t))
+                                      for index, t in steps], dtype=torch.float32, device=dev)
         st.t_table = torch.tensor([float(t) for _, t in steps], dtype=torch.float32, device=dev)
         st.ws = torch.empty(4 * b * ops.DDIM_PARTIALS, dtype=torch.float64, device=dev)
         if group is not None:
@@ -292,19 +354,34 @@ class DDIMSampler(object):
             st.ex(fn, args, dict(B=b, n=st.n))
 
     def _sample_fused(self, branches, img, time_range, total_steps, cfg_scale, phi, temperature, fs, callback,
-                      img_callback, log_every_t, intermediates, cfg_img=None, noise_generators=None):
+                      img_callback, log_every_t, intermediates, cfg_img=None, noise_generators=None, mask=None,
+                      x0=None, clean_cond=False):
         steps = [(total_steps - i - 1, time_range[i]) for i in range(total_steps)]
         st = self._fused_setup(branches[0], branches[1], tuple(img.shape), steps, cfg_scale, phi, temperature, fs,
-                               extra_branches=tuple(branches[2:]), cfg_img=cfg_img)
+                               extra_branches=tuple(branches[2:]), cfg_img=cfg_img,
+                               q_coefficients=mask is not None and not clean_cond)
         x = img.to(torch.float32).contiguous().clone()
         x_next = torch.empty_like(x)
         pred_x0 = torch.empty_like(x)
+        if mask is not None:
+            assert x0 is not None
+            # expanded once per call; the blend is then one tc_q_sample launch per step
+            mask = mask.to(device=st.dev, dtype=torch.float32).expand(x.shape).contiguous()
+            x0 = x0.to(device=st.dev, dtype=torch.float32).expand(x.shape).contiguous()
         if st.group is not None:
             from .distributed import sync_pair_state
             # same x_T on both ranks, and the same noise: from pair-rank 0's global RNG stream, or from the per-row
             # generators, which both ranks seed alike
             sync_pair_state(x, st.group, rng_state=noise_generators is None)
         for i, (index, _) in enumerate(steps):
+            if mask is not None:                                            # ddim.py:172-180, before the UNet
+                q_noise = None if clean_cond else randn_rows(x.shape, st.dev, noise_generators)
+                args = (x, x0, q_noise, mask, None if clean_cond else st.coef_table[i, st.q_off:])
+                kw = dict(B=st.b, n=st.n, clean=bool(clean_cond))
+                if st.ex is None:
+                    ops.q_sample(*args, **kw)
+                else:
+                    st.ex(ops.q_sample, args, kw)
             noise = randn_rows(x.shape, st.dev, noise_generators)          # one draw per step, as ddim.py:273
             self._fused_step(st, i, x, noise, x_next, pred_x0)
             x, x_next = x_next, x
