@@ -227,9 +227,35 @@ def ddim_step3(e_c, e_uc, e_img, x, noise, x_prev, pred_x0, coef, ws, *, B, n):
     ddim_step(e_c, e_uc, x, noise, x_prev, pred_x0, coef, ws, B=B, n=n, e_img=e_img)
 
 
+def video_u8(x16, x14, out, *, f_begin, f_end, out_frame):
+    """Middle-frame splice (inference.py:270), frame window, then the save path of inference.py:148-153 in torch."""
+    T = x16.shape[0]
+    v = x16.clone()
+    if x14 is not None:
+        v[T // 2 - 1:T // 2 + 1] = x14[T // 2 - 2:T // 2]
+    v = torch.clamp(v[f_begin:f_end].float(), -1.0, 1.0)
+    v = (v + 1.0) / 2.0
+    out[out_frame:out_frame + f_end - f_begin] = (v * 255).to(torch.uint8).permute(0, 2, 3, 1)
+
+
+def q_sample(x, x0, noise, mask, coef, *, B, n, clean=False):
+    """torch's fp32 arithmetic of ddpm3d.py:306-309 and ddim.py:172-180, in the reference's op order."""
+    xv = x.reshape(B, n)
+    x0v = x0.reshape(B, n)
+    if clean:
+        q = x0v.clone()
+    else:
+        c = coef[:2 * B].reshape(B, 2)
+        q = c[:, :1] * x0v + c[:, 1:] * noise.reshape(B, n)
+    if mask is not None:
+        m = mask.reshape(B, n)
+        q = q * m + (1.0 - m) * xv
+    xv.copy_(q)
+
+
 _TABLE = {f.__name__: f for f in (conv_gemm, groupnorm, row_stats, layernorm, attention, temporal_attention, softmax_rows, attention_wide,
                                   ncthw_to_cl, cl_to_ncthw, upsample2x, phase_split2, copy2d, add2d, time_embed,
-                                  small_linear, ddim_step, ddim_step3, gelu2d)}
+                                  small_linear, ddim_step, ddim_step3, gelu2d, video_u8, q_sample)}
 
 
 def executor(fn, args, kw):

@@ -1,14 +1,13 @@
 """world_size-2 gloo tests (CPU) of the N>1 path: clip sharding, the single weight broadcast, max-over-ranks."""
-import os
-import socket
 import sys
 from pathlib import Path
 
 import torch
 import torch.distributed as dist
-import torch.multiprocessing as mp
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+sys.path.insert(0, str(Path(__file__).resolve().parent))
+from distributed_harness import spawn  # noqa: E402
 from tooncrafter_b200 import distributed as D  # noqa: E402
 
 
@@ -23,16 +22,7 @@ def test_shard_clips_partition():
     assert D.clip_seed(123, 5) == 128
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _worker(rank, world, port, out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+def _worker(rank, world):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         torch.manual_seed(100 + rank)                            # different random weights per rank before the broadcast
@@ -46,31 +36,20 @@ def _worker(rank, world, port, out):
         clips = D.shard_clips(5, rank, world)
         allc = [None] * world
         dist.all_gather_object(allc, clips)
-        if rank == 0:
-            out.put(dict(sent=sent, sigs=gathered, mx=mx, clips=allc))
+        return dict(sent=sent, sigs=gathered, mx=mx, clips=allc)
     finally:
         dist.destroy_process_group()
 
 
 def test_two_rank_broadcast_and_timing_reduction():
-    world, port = 2, _free_port()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=120)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = spawn(_worker, world=2, timeout=120)[0]
     assert res["sent"] > 0
     assert res["sigs"][0] == res["sigs"][1]                     # every rank holds rank 0's weights and buffers
     assert res["mx"] == 11.0                                     # max over ranks, not the local value
     assert res["clips"] == [[0, 1, 2], [3, 4]]
 
 
-def _pair_worker(rank, world, port, out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+def _pair_worker(rank, world):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         group, pair, in_pair = D.latency_pairs()
@@ -83,24 +62,14 @@ def _pair_worker(rank, world, port, out):
         res = [None] * world
         dist.all_gather_object(res, dict(pair=pair, in_pair=in_pair, e_c=float(both[0].mean()), e_uc=float(both[1].mean()),
                                          x=float(x[0])))
-        if rank == 0:
-            out.put(res)
+        return res
     finally:
         dist.destroy_process_group()
 
 
 def test_latency_pairs_two_rank_exchange():
     """Latency mode plumbing on gloo: pair groups, the branch all-gather, the start-state broadcast."""
-    world, port = 2, _free_port()
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    procs = [ctx.Process(target=_pair_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    res = q.get(timeout=120)
-    for p in procs:
-        p.join(timeout=60)
-        assert p.exitcode == 0
+    res = spawn(_pair_worker, world=2, timeout=120)[0]
     assert [r["pair"] for r in res] == [0, 0] and [r["in_pair"] for r in res] == [0, 1]
     assert all(r["e_c"] == 0.0 and r["e_uc"] == 1.0 for r in res)        # slot 0 = conditional rank, slot 1 = unconditional
     assert all(r["x"] == 0.0 for r in res)                               # pair-rank 0's start latent wins

@@ -25,7 +25,8 @@ from tiny_config import TINY_T  # noqa: E402
 from tooncrafter_b200 import runtime  # noqa: E402
 from tooncrafter_b200.interpolate import get_parser, main, read_prompt_dir  # noqa: E402
 from tooncrafter_b200.modules import clip_tokenize  # noqa: E402
-from tooncrafter_b200.pipeline import ToonCrafterPipeline, check_n_samples, default_pairs_per_batch  # noqa: E402
+from tooncrafter_b200.pipeline import (ToonCrafterPipeline, check_count, check_n_samples,  # noqa: E402
+                                       default_pairs_per_batch)
 
 T = TINY_T
 
@@ -45,7 +46,7 @@ def pair_list(P, seed=13):
 
 
 class _Emulated:
-    """Runs the pipeline on the CPU program interpreter (pipeline_emulator), or on the GPU when dev is cuda."""
+    """Runs the pipeline on the CPU program interpreter (clip_emulator), or on the GPU when dev is cuda."""
 
     def __init__(self, pipe, dev):
         self.pipe, self.dev = pipe, dev
@@ -56,8 +57,8 @@ class _Emulated:
         def run(*a, **kw):
             if self.dev != "cpu":
                 return fn(*a, **kw).cpu()
-            import pipeline_emulator
-            runtime.TEST_EXECUTOR = pipeline_emulator.executor
+            import clip_emulator
+            runtime.TEST_EXECUTOR = clip_emulator.executor
             try:
                 return fn(*a, **kw)
             finally:
@@ -168,6 +169,21 @@ def test_invalid_n_samples_are_refused_before_any_work(bad):
         with pytest.raises(ValueError, match="n_samples"):
             pipe.animate(None, n_samples=bad)
     assert [check_n_samples(n) for n in (1, 2, np.int64(8))] == [1, 2, 8]
+
+
+@pytest.mark.parametrize("bad", [0, -1, True])
+def test_invalid_rows_per_batch_are_refused_before_any_work(bad):
+    """segments_per_batch of interpolate, animate and refine, and pairs_per_batch, with a model object that has
+    nothing but temporal_length: the check comes before any work."""
+    pipe = ToonCrafterPipeline(SimpleNamespace(temporal_length=16))
+    for call in (lambda: pipe.interpolate(None, segments_per_batch=bad),
+                 lambda: pipe.animate(None, segments_per_batch=bad),
+                 lambda: pipe.refine([None] * 16, 0.5, segments_per_batch=bad)):
+        with pytest.raises(ValueError, match="segments_per_batch must be an integer >= 1"):
+            call()
+    with pytest.raises(ValueError, match="pairs_per_batch must be an integer >= 1"):
+        pipe.interpolate_pairs([(None, None)], pairs_per_batch=bad)
+    assert [check_count(n, "pairs_per_batch") for n in (1, np.int64(3))] == [1, 3]
 
 
 def test_interpolate_pairs_refuses_bad_arguments_before_any_work():
@@ -282,6 +298,8 @@ def test_cli_arguments_of_n_samples_and_prompt_dir(tmp_path, capsys):
                 (["--prompt-dir", str(d), "--loop"], "--loop does not apply to --prompt-dir"),
                 (["--prompt-dir", str(d), "--prompt", "x"], "reads its prompts from the directory"),
                 (["--frames", "a.png", "b.png", "--text-input"], "apply to --prompt-dir"),
+                (["--frames", "a.png", "b.png", "--segments-per-batch", "0"], "segments_per_batch must be an integer"),
+                (["--prompt-dir", str(d), "--pairs-per-batch", "0"], "pairs_per_batch must be an integer >= 1"),
                 (["--prompt-dir", str(tmp_path / "none")], "not a directory"),
                 (["--frames", "a.png", "--prompt-dir", str(d)], "not allowed with"),
                 ([], "one of the arguments --frames --prompt-dir is required")]

@@ -12,12 +12,12 @@ HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE))
 sys.path.insert(0, str(HERE / "golden"))
 
-from test_pipeline_distributed_gpu import LATENCY_BOUND, VARIANTS, _init, _spawn  # noqa: E402
+from distributed_harness import LATENCY_BOUND  # noqa: E402
+from test_pipeline_distributed_gpu import VARIANTS, _init, _spawn  # noqa: E402
 
 
-def _worker(rank, world, port, out, one_gpu):
-    import traceback
-    dist, dev = _init(rank, world, port, one_gpu)
+def _worker(rank, world, one_gpu):
+    dist, dev = _init(rank, world, one_gpu)
     try:
         from test_pipeline import TINY_SIZE, keyframes, tiny_model
         from tooncrafter_b200.pipeline import ToonCrafterPipeline
@@ -38,10 +38,7 @@ def _worker(rank, world, port, out, one_gpu):
         r = ref["pairs_float"]
         res.update(latency_err=float((lat - r).abs().max()), scale=float(r.abs().max()),
                    latency_finite=bool(torch.isfinite(lat).all()), latency_sum=float(lat.double().sum()))
-        out.put((rank, res))
-    except BaseException:
-        out.put((rank, traceback.format_exc()))
-        raise
+        return res
     finally:
         dist.destroy_process_group()
 

@@ -81,14 +81,14 @@ _RUNS = {}
 
 def _emulated(K, loop=False, output="uint8", seed=123, frames=None, **kw):
     """One pipeline run on the tiny model through the CPU program interpreter (cached per argument set)."""
-    import pipeline_emulator
+    import clip_emulator
     key = (K, loop, output, seed, None if frames is None else tuple(frames), tuple(sorted(kw.items())))
     if key not in _RUNS:
         if "model" not in _RUNS:
             _RUNS["model"] = tiny_model()
         kf = keyframes(4 if frames is not None else K)
         kf = kf[list(frames)] if frames is not None else kf
-        runtime.TEST_EXECUTOR = pipeline_emulator.executor
+        runtime.TEST_EXECUTOR = clip_emulator.executor
         try:
             _RUNS[key] = ToonCrafterPipeline(_RUNS["model"]).interpolate(kf, steps=2, loop=loop, seed=seed,
                                                                          size=TINY_SIZE, output=output, **kw)
@@ -125,7 +125,7 @@ def test_rng_contract_on_the_general_sampler_path():
 
 
 def test_emulator_video_u8_matches_save_path_on_every_finite_half():
-    import pipeline_emulator
+    import ops_emulator
     h = torch.arange(-32768, 32768, dtype=torch.int32).to(torch.int16).view(torch.float16)
     h = h[torch.isfinite(h)]
     H, W = 16, 88
@@ -137,7 +137,7 @@ def test_emulator_video_u8_matches_save_path_on_every_finite_half():
     for xi, src in ((None, x16), (x14, spliced)):
         for f0, f1 in ((0, 16), (1, 16), (1, 15)):
             out = torch.full((20, H, W, 3), 77, dtype=torch.uint8)
-            pipeline_emulator.video_u8(x16, xi, out, f_begin=f0, f_end=f1, out_frame=3)
+            ops_emulator.video_u8(x16, xi, out, f_begin=f0, f_end=f1, out_frame=3)
             assert torch.equal(out[3:3 + f1 - f0], save_path_u8(src.permute(1, 0, 2, 3))[f0:f1])
             assert (out[:3] == 77).all() and (out[3 + f1 - f0:] == 77).all()
 

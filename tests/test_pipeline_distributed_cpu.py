@@ -1,14 +1,15 @@
-"""ToonCrafterPipeline with a process group, on the CPU program interpreter: two gloo ranks spawned by this file run the
-tiny model of test_pipeline.py, and every rank's returned video is compared with the single-process call, which rank 0
-makes afterwards (in a process with the same thread count: CPU matmuls round differently at other thread counts).
+"""ToonCrafterPipeline with a process group, on the CPU program interpreter: one session of two gloo ranks runs the tiny
+model of test_pipeline.py through interpolate (also at T = 8 frames per segment), animate, variants, interpolate_pairs
+and refine, and every rank's result is compared with the single-process call, which rank 0 makes afterwards (in a
+process with the same thread count: CPU matmuls round differently at other thread counts).
 
-With segments_per_batch=1 a sharded call is the single-process computation segment by segment (same per-segment
+With one row (or pair) per sample() call a sharded call is the single-process computation row by row (same per-row
 generators, same tower and encoder batches, same B = 1 sampling), so its output must be equal bit for bit.  Other
-batchings and latency mode change the batch rows of the UNet program and are held to the bounds the single-process
-tests apply to those."""
+batchings change the batch rows of the UNet program and are held to the bound the single-process tests apply to those;
+latency mode samples each guidance branch as its own program and is held to LATENCY_BOUND, both ranks of the pair
+returning the same bits."""
 import os
 import sys
-import traceback
 from pathlib import Path
 
 import pytest
@@ -18,27 +19,63 @@ HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE))
 sys.path.insert(0, str(HERE / "golden"))
 
+from distributed_harness import LATENCY_BOUND, spawn  # noqa: E402
 from test_pipeline import TINY_SIZE, _scale_close, keyframes, tiny_model  # noqa: E402
 from tooncrafter_b200 import runtime  # noqa: E402
 from tooncrafter_b200.pipeline import ToonCrafterPipeline  # noqa: E402
 
-# name -> (K, interpolate kwargs); K = 4 splits S = 3 segments into blocks [0, 1] / [2], as does K = 3 with loop
-CASES = {
-    "k4_u8": (4, dict(segments_per_batch=1)),
-    "k4_float": (4, dict(segments_per_batch=1, output="float")),
-    "k3_loop_u8": (3, dict(segments_per_batch=1, loop=True)),
-    "k3_loop_float": (3, dict(segments_per_batch=1, loop=True, output="float")),
-    "k4_default_batch_float": (4, dict(output="float")),
-}
-LATENCY_BOUND = 3e-2          # of the output scale: test_latency_gpu.py's bound for the pair against the fused path
+T8 = 8
 
 
-def _interpolate(pipe, K, kw):
-    return pipe.interpolate(keyframes(K), steps=2, seed=123, size=TINY_SIZE, **kw)
+def _interpolate(K, **kw):
+    return lambda pipe: pipe.interpolate(keyframes(K), steps=2, seed=123, size=TINY_SIZE, **kw)
 
 
 def _animate(pipe):
     return pipe.animate(keyframes(1, seed=5)[0], steps=2, seed=77, size=TINY_SIZE)
+
+
+def _variants(output):
+    """n_samples=3 on K = 2: three rows, blocks [0, 1] / [2]."""
+    return lambda pipe: pipe.interpolate(keyframes(2, seed=8), steps=1, seed=21, size=TINY_SIZE, n_samples=3,
+                                         segments_per_batch=1, output=output)
+
+
+def _pairs(output):
+    """P = 3 pairs, blocks [0, 1] / [2]."""
+    def call(pipe):
+        kf = keyframes(6, seed=9)
+        return pipe.interpolate_pairs([(kf[2 * i], kf[2 * i + 1]) for i in range(3)], n_samples=2, steps=1, seed=33,
+                                      size=TINY_SIZE, pairs_per_batch=1, output=output)
+    return call
+
+
+def _refine(output):
+    """n_samples=3 with keep: three rows, blocks [0, 1] / [2]."""
+    return lambda pipe: pipe.refine(keyframes(8, seed=12), 0.5, keep=[0, 1, 7], steps=2, seed=21, size=TINY_SIZE,
+                                    n_samples=3, segments_per_batch=1, output=output)
+
+
+# name -> call, made on the sharded pipeline and by rank 0 on the single-process one; K = 4 splits S = 3 segments into
+# blocks [0, 1] / [2], as does K = 3 with loop (with the closing seam)
+CASES = {
+    "k4_u8": _interpolate(4, segments_per_batch=1),
+    "k4_float": _interpolate(4, segments_per_batch=1, output="float"),
+    "k3_loop_u8": _interpolate(3, segments_per_batch=1, loop=True),
+    "k3_loop_float": _interpolate(3, segments_per_batch=1, loop=True, output="float"),
+    "k4_default_batch_float": _interpolate(4, output="float"),
+    "animate": _animate,
+    "t8_k3_loop_u8": _interpolate(3, segments_per_batch=1, loop=True, video_length=T8),
+    "variants_u8": _variants("uint8"), "variants_float": _variants("float"),
+    "pairs_u8": _pairs("uint8"), "pairs_float": _pairs("float"),
+    "refine_u8": _refine("uint8"), "refine_float": _refine("float"),
+}
+# name -> call, made on the latency-mode pipeline; its single-process reference is CASES[name] or SINGLE[name]
+LATENCY = {"k4_float": CASES["k4_float"], "animate": _animate,
+           "t8_k4_float": _interpolate(4, segments_per_batch=1, output="float", video_length=T8),
+           "variants_float": CASES["variants_float"], "pairs_float": CASES["pairs_float"],
+           "refine_float": CASES["refine_float"]}
+SINGLE = {"t8_k4_float": LATENCY["t8_k4_float"]}
 
 
 def _refusal(fn):
@@ -49,88 +86,64 @@ def _refusal(fn):
     return None
 
 
-def _worker(rank, world, port, out):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+def _worker(rank, world):
     import torch.distributed as dist
 
-    import pipeline_emulator
+    import clip_emulator
     torch.set_num_threads(max(1, (os.cpu_count() or 2) // world))
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        runtime.TEST_EXECUTOR = pipeline_emulator.executor
+        runtime.TEST_EXECUTOR = clip_emulator.executor
         m = tiny_model()
         group = dist.group.WORLD
-        res = {}
         pipe = ToonCrafterPipeline(m, group)
-        for name, (K, kw) in CASES.items():
-            res[name] = _interpolate(pipe, K, kw).numpy()
-        res["animate"] = _animate(pipe).numpy()
+        res = {name: fn(pipe).numpy() for name, fn in CASES.items()}
         lat = ToonCrafterPipeline(m, group, latency=True)
-        res["latency_k4_float"] = _interpolate(lat, 4, dict(segments_per_batch=1, output="float")).numpy()
-        res["latency_animate"] = _animate(lat).numpy()
-        res["refuse_cfg_img"] = _refusal(lambda: _interpolate(lat, 3, dict(cfg_img=5.0)))
-        res["refuse_cfg_scale_1"] = _refusal(lambda: _interpolate(lat, 3, dict(cfg_scale=1.0)))
+        res.update({"latency_" + name: fn(lat).numpy() for name, fn in LATENCY.items()})
+        res["refuse_cfg_img"] = _refusal(lambda: _interpolate(3, cfg_img=5.0)(lat))
+        res["refuse_cfg_scale_1"] = _refusal(lambda: _interpolate(3, cfg_scale=1.0)(lat))
         res["refuse_no_group"] = _refusal(lambda: ToonCrafterPipeline(m, latency=True))
         one = dist.new_group(ranks=[0])                       # a group of odd size (collective: every rank calls it)
         if rank == 0:
             res["refuse_odd_world"] = _refusal(lambda: ToonCrafterPipeline(m, one, latency=True))
         # group=None with torch.distributed initialised: the single-process call, no collective
-        res["no_group"] = _interpolate(ToonCrafterPipeline(m), 4, dict(segments_per_batch=1, output="float")).numpy()
+        res["no_group"] = CASES["k4_float"](ToonCrafterPipeline(m)).numpy()
         if rank == 0:
             single = ToonCrafterPipeline(m)
-            for name, (K, kw) in CASES.items():
-                res["single_" + name] = _interpolate(single, K, kw).numpy()
-            res["single_animate"] = _animate(single).numpy()
-        out.put((rank, res))
-    except BaseException:
-        out.put((rank, traceback.format_exc()))
-        raise
+            res.update({"single_" + name: fn(single).numpy() for name, fn in {**CASES, **SINGLE}.items()})
+        return res
     finally:
         runtime.TEST_EXECUTOR = None
         dist.destroy_process_group()
 
 
-def _free_port():
-    import socket
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 @pytest.fixture(scope="module")
 def sharded():
     """{case: [rank 0's result, rank 1's result]} of one world-2 session; "single_<case>": [the single-process call]."""
-    import torch.multiprocessing as mp
-    world = 2
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, q)) for r in range(world)]
-    for p in procs:
-        p.start()
-    try:
-        got = dict(q.get(timeout=2400) for _ in range(world))
-    finally:
-        for p in procs:
-            p.join(timeout=120)
-            if p.is_alive():
-                p.kill()
-                p.join()
-    for r in range(world):
-        assert isinstance(got[r], dict), f"rank {r} failed:\n{got[r]}"
-    assert all(p.exitcode == 0 for p in procs)
+    got = spawn(_worker, world=2)
     return {name: [torch.from_numpy(got[r][name]) if hasattr(got[r][name], "dtype") else got[r][name]
-                   for r in range(world) if name in got[r]] for name in got[0]}
+                   for r in range(2) if name in got[r]] for name in got[0]}
 
 
-@pytest.mark.parametrize("case", [c for c in CASES if "default" not in c])
-def test_sharded_segments_equal_single_process(sharded, case):
+def _check_equal(sharded, case, shape=None):
     ref, = sharded["single_" + case]
+    assert shape is None or tuple(ref.shape) == shape, (case, tuple(ref.shape))
     for r, got in enumerate(sharded[case]):
         assert got.shape == ref.shape and got.dtype == ref.dtype, (case, r)
         assert torch.equal(got, ref), f"{case}: rank {r} differs from the single-process call"
+
+
+def _check_latency(sharded, case):
+    ref, = sharded["single_" + case]
+    a, b = sharded["latency_" + case]
+    assert torch.equal(a, b), "the two ranks of the pair returned different results"
+    assert a.shape == ref.shape
+    _scale_close(a, ref, f"latency mode {case} vs single process", rel=LATENCY_BOUND)
+
+
+@pytest.mark.parametrize("case", ["k4_u8", "k4_float", "k3_loop_u8", "k3_loop_float"])
+def test_sharded_segments_equal_single_process(sharded, case):
+    _check_equal(sharded, case)
 
 
 def test_sharded_default_batching_matches_single_process(sharded):
@@ -143,21 +156,13 @@ def test_sharded_default_batching_matches_single_process(sharded):
 
 
 def test_sharded_animate_equals_single_process(sharded):
-    ref, = sharded["single_animate"]
-    for r, got in enumerate(sharded["animate"]):
-        assert torch.equal(got, ref), f"animate: rank {r} differs from the single-process call"
+    _check_equal(sharded, "animate")
 
 
 def test_latency_mode_matches_single_process(sharded):
     """One GPU pair samples all 3 segments, one guidance branch per rank; pair-rank 0 decodes and broadcasts."""
-    ref, = sharded["single_k4_float"]
-    a, b = sharded["latency_k4_float"]
-    assert torch.equal(a, b), "the two ranks of the pair returned different videos"
-    _scale_close(a, ref, "latency mode K=4 vs single process", rel=LATENCY_BOUND)
-    ref, = sharded["single_animate"]
-    a, b = sharded["latency_animate"]
-    assert torch.equal(a, b) and a.shape == ref.shape
-    _scale_close(a, ref, "latency mode animate vs single process", rel=LATENCY_BOUND)
+    _check_latency(sharded, "k4_float")
+    _check_latency(sharded, "animate")
 
 
 def test_latency_mode_refusals(sharded):
@@ -177,3 +182,35 @@ def test_no_group_is_the_single_process_call(sharded):
     ref, = sharded["single_k4_float"]
     for got in sharded["no_group"]:
         assert torch.equal(got, ref)
+
+
+@pytest.mark.parametrize("case", ["k3_loop_u8"])
+def test_sharded_video_length_equals_single_process(sharded, case):
+    """At a clip length other than the model's temporal_length."""
+    _check_equal(sharded, "t8_" + case, ((T8 - 1) * 3, *TINY_SIZE, 3))
+
+
+def test_latency_mode_video_length_matches_single_process(sharded):
+    _check_latency(sharded, "t8_k4_float")
+    assert sharded["latency_t8_k4_float"][0].shape == (3, 3, T8, *TINY_SIZE)
+
+
+@pytest.mark.parametrize("case", ["variants_u8", "variants_float", "pairs_u8", "pairs_float"])
+def test_sharded_rows_and_pairs_equal_single_process(sharded, case):
+    expect = {"variants_u8": (3, 4, *TINY_SIZE, 3), "variants_float": (3, 1, 3, 4, *TINY_SIZE),
+              "pairs_u8": (3, 2, 4, *TINY_SIZE, 3), "pairs_float": (3, 2, 3, 4, *TINY_SIZE)}[case]
+    _check_equal(sharded, case, expect)
+
+
+@pytest.mark.parametrize("case", ["variants_float", "pairs_float"])
+def test_latency_mode_rows_and_pairs_match_single_process(sharded, case):
+    _check_latency(sharded, case)
+
+
+@pytest.mark.parametrize("case", ["u8", "float"])
+def test_sharded_refine_equals_single_process(sharded, case):
+    _check_equal(sharded, "refine_" + case, (3, 8, *TINY_SIZE, 3) if case == "u8" else (3, 3, 8, *TINY_SIZE))
+
+
+def test_latency_mode_refine_matches_single_process(sharded):
+    _check_latency(sharded, "refine_float")

@@ -3,9 +3,7 @@ one GPU over gloo (collectives staged through host memory), and two GPUs over NC
 Every rank compares its returned video with the single-process pipeline run in the same process afterwards: equal bit
 for bit with segments_per_batch=1, within test_latency_gpu.py's bound in latency mode.  The full-size case runs on two
 GPUs only."""
-import os
 import sys
-import traceback
 from pathlib import Path
 
 import pytest
@@ -15,12 +13,12 @@ HERE = Path(__file__).resolve().parent
 sys.path.insert(0, str(HERE))
 sys.path.insert(0, str(HERE / "golden"))
 
+from distributed_harness import LATENCY_BOUND, spawn  # noqa: E402
+
 VARIANTS = dict(argnames="one_gpu", argvalues=[True, False], ids=["two_ranks_on_one_gpu_gloo", "two_gpus_nccl"])
-LATENCY_BOUND = 3e-2          # of the output scale, as test_latency_mode_matches_single_gpu_fused_path
 
 
-def _init(rank, world, port, one_gpu):
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+def _init(rank, world, one_gpu):
     import torch.distributed as dist
     dev = torch.device("cuda", 0 if one_gpu else rank)
     torch.cuda.set_device(dev)
@@ -32,8 +30,8 @@ def _init(rank, world, port, one_gpu):
     return dist, dev
 
 
-def _tiny_worker(rank, world, port, out, one_gpu):
-    dist, dev = _init(rank, world, port, one_gpu)
+def _tiny_worker(rank, world, one_gpu):
+    dist, dev = _init(rank, world, one_gpu)
     try:
         from test_pipeline import TINY_SIZE, keyframes, tiny_model
         from tooncrafter_b200.pipeline import ToonCrafterPipeline
@@ -48,16 +46,13 @@ def _tiny_worker(rank, world, port, out, one_gpu):
         res = {f"equal_{o}": bool(got[o].shape == ref[o].shape and torch.equal(got[o], ref[o])) for o in got}
         res.update(latency_err=float((lat - ref["float"]).abs().max()), scale=float(ref["float"].abs().max()),
                    latency_finite=bool(torch.isfinite(lat).all()), latency_sum=float(lat.double().sum()))
-        out.put((rank, res))
-    except BaseException:
-        out.put((rank, traceback.format_exc()))
-        raise
+        return res
     finally:
         dist.destroy_process_group()
 
 
-def _full_size_worker(rank, world, port, out, one_gpu):
-    dist, dev = _init(rank, world, port, one_gpu)
+def _full_size_worker(rank, world, one_gpu):
+    dist, dev = _init(rank, world, one_gpu)
     try:
         from test_pipeline import keyframes
         from tiny_config import FULL_DDCONFIG, FULL_UNET, model_config
@@ -80,46 +75,17 @@ def _full_size_worker(rank, world, port, out, one_gpu):
         kw = dict(steps=2, segments_per_batch=1, output="float")
         got = ToonCrafterPipeline(m, dist.group.WORLD).interpolate(kf, **kw)
         ref = ToonCrafterPipeline(m).interpolate(kf, **kw)
-        out.put((rank, dict(equal=bool(got.shape == ref.shape and torch.equal(got, ref)),
-                            finite=bool(torch.isfinite(got).all()), shape=tuple(got.shape))))
-    except BaseException:
-        out.put((rank, traceback.format_exc()))
-        raise
+        return dict(equal=bool(got.shape == ref.shape and torch.equal(got, ref)),
+                    finite=bool(torch.isfinite(got).all()), shape=tuple(got.shape))
     finally:
         dist.destroy_process_group()
 
 
-def _free_port():
-    import socket
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _spawn(worker, one_gpu, timeout):
-    """Run `worker` on two ranks; {rank: its result dict}."""
+    """Run worker(rank, 2, one_gpu) on two ranks; {rank: its result dict}."""
     if not one_gpu and torch.cuda.device_count() < 2:
         pytest.skip("the NCCL variant shards over two GPUs")
-    import torch.multiprocessing as mp
-    ctx = mp.get_context("spawn")
-    q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=worker, args=(r, 2, port, q, one_gpu)) for r in range(2)]
-    for p in procs:
-        p.start()
-    try:
-        res = dict(q.get(timeout=timeout) for _ in procs)
-    finally:
-        for p in procs:
-            p.join(timeout=120)
-            if p.is_alive():
-                p.kill()
-                p.join()
-    for r in range(2):
-        assert isinstance(res[r], dict), f"rank {r} failed:\n{res[r]}"
-    assert all(p.exitcode == 0 for p in procs)
+    res = spawn(worker, one_gpu, world=2, timeout=timeout)
     print(worker.__name__, res)
     return res
 

@@ -204,7 +204,7 @@ def test_animate_on_emulator_follows_image_guided_synthesis_and_its_rng_contract
     m = tiny_model(first_stage)
     image = keyframes(1, seed=5)[0]
     pipe = ToonCrafterPipeline(m)
-    runtime.TEST_EXECUTOR = __import__("pipeline_emulator").executor
+    runtime.TEST_EXECUTOR = __import__("clip_emulator").executor
     try:
         u8 = pipe.animate(image, steps=2, seed=77, size=TINY_SIZE)
         vf = pipe.animate(image, steps=2, seed=77, size=TINY_SIZE, output="float")
@@ -228,13 +228,13 @@ def test_animate_on_emulator_follows_image_guided_synthesis_and_its_rng_contract
 def test_interpolate_with_plain_first_stage_decodes_each_segment_once():
     """K = 3 on the plain first stage: one T-frame decode per segment and no T - 2 frame decode (recorded launches),
     and the joined video follows the seam rule of the float output."""
-    import pipeline_emulator
+    import clip_emulator
     m = tiny_model("plain")
     kf = keyframes(3, seed=8)
     pipe = ToonCrafterPipeline(m)
     m.first_stage_model._dec_engine = None                # drop plans other tests made on the shared model
     log = []
-    runtime.TEST_EXECUTOR = _recording(pipeline_emulator.executor, log)
+    runtime.TEST_EXECUTOR = _recording(clip_emulator.executor, log)
     try:
         u8 = pipe.interpolate(kf, steps=2, seed=5, size=TINY_SIZE)
         vf = pipe.interpolate(kf, steps=2, seed=5, size=TINY_SIZE, output="float")

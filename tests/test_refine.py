@@ -22,7 +22,7 @@ from tiny_config import TINY_T, TINY_UNET, model_config  # noqa: E402
 
 from oracle import ddim_oracle, unet_oracle  # noqa: E402
 from tooncrafter_b200 import diffusion, layout, runtime, synthetic  # noqa: E402
-from tooncrafter_b200.pipeline import ToonCrafterPipeline  # noqa: E402
+from tooncrafter_b200.pipeline import ToonCrafterPipeline, preprocess  # noqa: E402
 from tooncrafter_b200.sampler import DDIMSampler, DDIMSamplerMultiCond  # noqa: E402
 
 GOLD = np.load(HERE / "golden" / "refine_tiny.npz")
@@ -144,16 +144,16 @@ class _Forced:
 def _run(m, cls, fused, fn):
     """fn(sampler) on the fused path (program interpreter) or the general path (apply_model through the same
     interpreted engine)."""
-    import refine_emulator
+    import clip_emulator
     unet = m.model.diffusion_model
     s = cls(m)
     saved = unet.forward
     if fused:
-        s._test_executor = refine_emulator.executor
+        s._test_executor = clip_emulator.executor
     else:
         s._test_executor = None
         unet.forward = lambda x, t, context=None, fs=None, **kw: unet._engine.forward(
-            x, t, context, fs, executor=refine_emulator.executor).clone()
+            x, t, context, fs, executor=clip_emulator.executor).clone()
     try:
         return fn(s)
     finally:
@@ -223,7 +223,7 @@ def test_multicond_decode_raises_key_error_as_the_reference(tiny_model):
 def test_fused_blend_touches_only_masked_frames(tiny_model):
     """One step from a constant latent with a binary frame mask and clean_cond: after the fused path's tc_q_sample the
     latent holds x0 on the masked frames and is unchanged elsewhere."""
-    import refine_emulator
+    import clip_emulator
     gi = refine_inputs()
     x_T = torch.full_like(gi["x_T"], 0.25)
     mask = torch.zeros(1, 1, T, 1, 1)
@@ -231,7 +231,7 @@ def test_fused_blend_touches_only_masked_frames(tiny_model):
     seen = []
 
     def spy(fn, args, kw):
-        refine_emulator.executor(fn, args, kw)
+        clip_emulator.executor(fn, args, kw)
         if fn.__name__ == "q_sample":
             seen.append(args[0].clone())
 
@@ -258,7 +258,7 @@ def test_t_start_is_checked(tiny_model):
 
 # ----------------------------------------------------------------------------------------- pipeline
 class Emulated:
-    """A pipeline run on the CPU program interpreter with q_sample (refine_emulator), or on the GPU when dev is cuda;
+    """A pipeline run on the CPU program interpreter (clip_emulator), or on the GPU when dev is cuda;
     results come back on the CPU."""
 
     def __init__(self, pipe, dev="cpu"):
@@ -270,8 +270,8 @@ class Emulated:
         def run(*a, **kw):
             if self.dev != "cpu":
                 return fn(*a, **kw).cpu()
-            import refine_emulator
-            runtime.TEST_EXECUTOR = refine_emulator.executor
+            import clip_emulator
+            runtime.TEST_EXECUTOR = clip_emulator.executor
             try:
                 return fn(*a, **kw)
             finally:
@@ -325,10 +325,10 @@ def test_refine_encodes_interior_frames_in_decode_chunks():
     does not depend on the chunking."""
     m = model("dualref", "cpu")
     p = ToonCrafterPipeline(m)
-    import pipeline_emulator
+    import clip_emulator
     clip = keyframes(8, seed=73)
-    frames = p._preprocess(clip, TINY_SIZE, "uint8")
-    runtime.TEST_EXECUTOR = pipeline_emulator.executor
+    frames = preprocess(clip, TINY_SIZE)
+    runtime.TEST_EXECUTOR = clip_emulator.executor
     seen = []
     enc = m.first_stage_model.encode
     try:

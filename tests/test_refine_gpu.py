@@ -179,11 +179,9 @@ def test_refine_full_size(cuda_tf32_off, full_models, first_stage):
     assert not torch.equal(keep, one)
 
 
-def _worker(rank, world, port, out, one_gpu):
-    import traceback
-
+def _worker(rank, world, one_gpu):
     from test_pipeline_distributed_gpu import _init
-    dist, dev = _init(rank, world, port, one_gpu)
+    dist, dev = _init(rank, world, one_gpu)
     try:
         from test_pipeline import TINY_SIZE, tiny_model
         from tooncrafter_b200.pipeline import ToonCrafterPipeline
@@ -195,12 +193,9 @@ def _worker(rank, world, port, out, one_gpu):
         lat = ToonCrafterPipeline(m, dist.group.WORLD, latency=True).refine(clip, 0.75, output="float", **kw)
         single = ToonCrafterPipeline(m)
         ref, ref_f = single.refine(clip, 0.75, **kw), single.refine(clip, 0.75, output="float", **kw)
-        out.put((rank, dict(equal=bool(torch.equal(got, ref)), equal_float=bool(torch.equal(got_f, ref_f)),
-                            latency_err=float((lat - ref_f).abs().max()), scale=float(ref_f.abs().max()),
-                            latency_sum=float(lat.double().sum()))))
-    except BaseException:
-        out.put((rank, traceback.format_exc()))
-        raise
+        return dict(equal=bool(torch.equal(got, ref)), equal_float=bool(torch.equal(got_f, ref_f)),
+                    latency_err=float((lat - ref_f).abs().max()), scale=float(ref_f.abs().max()),
+                    latency_sum=float(lat.double().sum()))
     finally:
         dist.destroy_process_group()
 
@@ -209,7 +204,8 @@ def _worker(rank, world, port, out, one_gpu):
 def test_refine_two_ranks_on_one_gpu_equal_single_process():
     """n_samples=3 with keep over two gloo ranks (rows [0, 1] / [2]): bit for bit; latency mode within its bound and
     the same on both ranks."""
-    from test_pipeline_distributed_gpu import LATENCY_BOUND, _spawn
+    from distributed_harness import LATENCY_BOUND
+    from test_pipeline_distributed_gpu import _spawn
     res = _spawn(_worker, True, 900)
     for r in range(2):
         assert res[r]["equal"] and res[r]["equal_float"], res[r]

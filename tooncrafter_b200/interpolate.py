@@ -224,20 +224,18 @@ def read_init_video(path: str) -> np.ndarray:
 
 def parse_frame_ranges(spec: str, T: int) -> list:
     """--keep-frames: comma-separated frame indices and inclusive ranges a-b ("0-3,12-15"), each within 0 .. T-1 and
-    listed once.  ValueError otherwise."""
+    listed once (ToonCrafterPipeline.refine's keep, sorted).  ValueError otherwise."""
+    from .pipeline import check_keep
     out = []
     for part in spec.split(","):
         part = part.strip()
         if not re.fullmatch(r"\d+(-\d+)?", part):
             raise ValueError(f"--keep-frames: {part!r} is not a frame index or a range a-b")
         a, _, b = part.partition("-")
-        lo, hi = int(a), int(b or a)
-        if not 0 <= lo <= hi < T:
-            raise ValueError(f"--keep-frames: {part!r} is not within frames 0 .. {T - 1}")
-        out.extend(range(lo, hi + 1))
-    if len(set(out)) != len(out):
-        raise ValueError(f"--keep-frames: {spec!r} lists a frame twice")
-    return out
+        if int(a) > int(b or a):
+            raise ValueError(f"--keep-frames: {part!r} is not a range a-b with a <= b")
+        out.extend(range(int(a), int(b or a) + 1))
+    return check_keep(out, T)
 
 
 def read_prompts(args, n_segments: int):
@@ -277,14 +275,15 @@ def main(argv=None) -> int:
     args = ap.parse_args(argv)
     if args.frames is None and args.prompt_dir is None and args.init_video is None:
         ap.error("one of the arguments --frames --prompt-dir is required (or --init-video to refine a clip)")
-    from .pipeline import check_n_samples, check_video_length
+    from .pipeline import check_count, check_n_samples, check_strength, check_video_length
     try:
         if args.video_length is not None:
             check_video_length(args.video_length)
         if args.n_samples is not None:
             check_n_samples(args.n_samples)
-        if args.pairs_per_batch is not None and args.pairs_per_batch < 1:
-            raise ValueError(f"--pairs-per-batch must be at least 1, got {args.pairs_per_batch}")
+        for name in ("segments_per_batch", "pairs_per_batch"):
+            if getattr(args, name) is not None:
+                check_count(getattr(args, name), name)
     except ValueError as e:
         ap.error(str(e))
     if args.prompt_dir is not None:
@@ -309,9 +308,7 @@ def main(argv=None) -> int:
             T = check_video_length(len(args.clip))
             if args.video_length is not None and args.video_length != T:
                 raise ValueError(f"--video-length {args.video_length}: the clip has {T} frames")
-            if not 0.0 < args.strength <= 1.0 or int(args.strength * args.ddim_steps) < 1:
-                raise ValueError(f"--strength {args.strength} x --ddim-steps {args.ddim_steps} runs no DDIM step; "
-                                 "give a strength in (0, 1]")
+            check_strength(args.strength, args.ddim_steps)
             if args.keep_frames is not None:
                 args.keep = parse_frame_ranges(args.keep_frames, T)
         except ValueError as e:

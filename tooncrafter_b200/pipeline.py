@@ -65,7 +65,7 @@ the same way (each rank encoding only its own groups) and broadcasts each block'
 """
 from __future__ import annotations
 
-from typing import Optional, Sequence, Union
+from typing import NamedTuple, Optional, Sequence, Union
 
 import numpy as np
 import torch
@@ -132,11 +132,98 @@ def default_pairs_per_batch(size, T: int, n_samples: int) -> int:
 VARIANT_SEED_STRIDE = 2 ** 32 + 0x9E3779B9
 
 
+def check_count(value, name: str) -> int:
+    """n_samples, segments_per_batch, pairs_per_batch: an integer >= 1 (numpy integers too); bools are refused."""
+    if isinstance(value, bool) or not isinstance(value, (int, np.integer)) or value < 1:
+        raise ValueError(f"{name} must be an integer >= 1, got {value!r}")
+    return int(value)
+
+
 def check_n_samples(n) -> int:
     """Variants per input (the reference's --n_samples): an integer >= 1; bools are refused."""
-    if isinstance(n, bool) or not isinstance(n, (int, np.integer)) or n < 1:
-        raise ValueError(f"n_samples must be an integer >= 1, got {n!r}")
-    return int(n)
+    return check_count(n, "n_samples")
+
+
+def check_strength(strength, steps: int) -> int:
+    """refine's DDIM steps: k = int(strength * steps) for a strength in (0, 1]; ValueError when k < 1."""
+    if (isinstance(strength, bool) or not isinstance(strength, (int, float, np.integer, np.floating))
+            or not 0.0 < strength <= 1.0):
+        raise ValueError(f"strength must be a number in (0, 1], got {strength!r}")
+    k = int(strength * steps)
+    if k < 1:
+        raise ValueError(f"strength {strength} x steps {steps} runs no DDIM step (int(strength * steps) < 1)")
+    return k
+
+
+def check_keep(keep, T: int) -> Optional[list]:
+    """refine's kept frames: None, or frame indices from 0 to T - 1, each listed once.  Returns them sorted (None for
+    an empty list)."""
+    if keep is None:
+        return None
+    keep = list(keep)
+    if any(isinstance(j, bool) or not isinstance(j, (int, np.integer)) or not 0 <= j < T for j in keep):
+        raise ValueError(f"keep must hold frame indices from 0 to {T - 1}, got {keep!r}")
+    if len(set(int(j) for j in keep)) != len(keep):
+        raise ValueError(f"keep lists a frame twice: {keep!r}")
+    return sorted(int(j) for j in keep) or None
+
+
+class _Call(NamedTuple):
+    T: int                      # frames per segment
+    n: int                      # variants per input
+    per_batch: int              # segments_per_batch (rows per sample() call), or interpolate_pairs' pairs_per_batch
+    variant_axis: bool          # the result keeps its leading variant axis (n_samples was given)
+    size: tuple
+    output: str
+    steps: int
+    cfg_scale: float
+    eta: float
+    fs: int
+    guidance_rescale: float
+    timestep_spacing: str
+    cfg_img: Optional[float]
+
+
+class _Row(NamedTuple):
+    """One sampled row: a (segment, variant), or a (pair, variant) of interpolate_pairs."""
+    seg: int                    # its segment: an index into the first / last keyframe lists of the call that samples it
+    seed: int                   # the seed of its device generator (x_T and step noise)
+    index: int                  # float output: its clip in the flattened [rows, 3, T, H, W] video
+    f_begin: int                # uint8 output: its frames f_begin .. f_end - 1 (the seam rule) go to frames out_frame ..
+    f_end: int                  # of the flattened [frames, H, W, 3] video
+    out_frame: int
+
+
+class _Refine(NamedTuple):
+    """refine's start: one segment whose keyframes 0 and 1 are the clip's first and last frames."""
+    frames: torch.Tensor        # the preprocessed frames 1 .. T-2
+    seeds: list                 # their posterior-noise seeds
+    k: int                      # DDIM steps to run
+    keep: Optional[list]        # frame indices held to the clip, or None
+
+
+def _check_prompts(prompts, count: int, what: str) -> None:
+    """One string, a list of `count` strings, or token ids [count, 77]: one prompt per segment or pair (`what`)."""
+    if isinstance(prompts, torch.Tensor):
+        if prompts.dim() != 2 or prompts.shape[0] != count:
+            raise ValueError(f"token ids must be [{count} {what}, 77], got {tuple(prompts.shape)}")
+    elif not isinstance(prompts, str) and len(prompts) != count:
+        raise ValueError(f"{len(prompts)} prompts for {count} {what}")
+
+
+def _span(rows, output: str) -> tuple:
+    """[begin, end) of the flattened output that the consecutive `rows` write."""
+    a, b = rows[0], rows[-1]
+    if output == "float":
+        return a.index, b.index + 1
+    return a.out_frame, b.out_frame + b.f_end - b.f_begin
+
+
+def _posterior_sample(m, post, seeds) -> torch.Tensor:
+    """First-stage latents of an encoded batch, frame i's posterior noise from a CPU generator seeded seeds[i]."""
+    noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(s))
+                         for s in seeds])
+    return m.get_first_stage_encoding(post, noise=noise)
 
 
 def _decode_chunks(dec, lat, n: int, ref, ex):
@@ -178,27 +265,6 @@ class ToonCrafterPipeline:
         elif group is not None:
             self._block, self._n_blocks = dist.get_rank(group), dist.get_world_size(group)
 
-    def _owner(self, block: int) -> int:
-        """Global rank that holds block `block`'s result: the rank, or pair-rank 0 of the pair, that computes it."""
-        return dist.get_global_rank(self.group, 2 * block if self.latency else block)
-
-    def _text(self, prompts, S: int):
-        """(per-segment text embeddings [S, 77, D], the embedding of "" [1, 77, D]) from one text-tower pass."""
-        m = self.model
-        if isinstance(prompts, torch.Tensor):
-            if prompts.dim() != 2 or prompts.shape[0] != S:
-                raise ValueError(f"token ids must be [S={S}, 77], got {tuple(prompts.shape)}")
-            uniq, inv = torch.unique(prompts.long().cpu(), dim=0, return_inverse=True)
-            emb = m.get_learned_conditioning(torch.cat([uniq, clip_tokenize([""], prompts.shape[1])]).to(m.device))
-            return emb[inv.to(emb.device)], emb[-1:]
-        texts = [prompts] * S if isinstance(prompts, str) else list(prompts)
-        if len(texts) != S:
-            raise ValueError(f"{len(texts)} prompts for {S} segments")
-        distinct = list(dict.fromkeys(texts + [""]))
-        emb = m.get_learned_conditioning(distinct)
-        idx = torch.tensor([distinct.index(t) for t in texts], device=emb.device)
-        return emb[idx], emb[distinct.index("")][None]
-
     @torch.no_grad()
     def interpolate(self, keyframes, prompts: Union[str, Sequence[str], torch.Tensor] = "", steps: int = 50,
                     cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
@@ -220,19 +286,14 @@ class ToonCrafterPipeline:
         output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]].
         With an integer n_samples both gain a leading variant axis, [n, F, H, W, 3] / [n, S, 3, T, H, W], and
         video[v] is a complete single-sample result (video[0] is the n_samples=None result)."""
-        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
-        n = 1 if n_samples is None else check_n_samples(n_samples)
-        if segments_per_batch is None:
-            segments_per_batch = default_segments_per_batch(size, T)
-        frames = self._preprocess(keyframes, size, output)
+        c = self._checked(video_length, n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
+                          guidance_rescale, timestep_spacing, cfg_img)
+        frames = preprocess(keyframes, c.size, self.model.device)
         K = frames.shape[0]
         if K < 2:
             raise ValueError("interpolation needs at least two keyframes")
         S = K if loop else K - 1
-        video = self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, loop, seed, n,
-                               segments_per_batch, output, T,
-                               _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img))
-        return video if n_samples is not None else video[0]
+        return self._generate(frames, prompts, list(range(S)), [(k + 1) % K for k in range(S)], True, loop, seed, c)
 
     @torch.no_grad()
     def animate(self, image, prompt: Union[str, torch.Tensor] = "", steps: int = 50, cfg_scale: float = 7.5,
@@ -250,16 +311,10 @@ class ToonCrafterPipeline:
 
         Returns uint8 [T, size[0], size[1], 3] on the model's device; with output="float", the spliced video before
         quantisation, float32 [3, T, size[0], size[1]]; with an integer n_samples, [n, T, H, W, 3] / [n, 3, T, H, W]."""
-        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
-        n = 1 if n_samples is None else check_n_samples(n_samples)
-        if segments_per_batch is None:
-            segments_per_batch = default_segments_per_batch(size, T)
-        frames = self._preprocess([image], size, output)
-        video = self._generate(frames, prompt, [0], [0], False, False, seed, n, segments_per_batch, output, T,
-                               _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img))
-        if output == "float":
-            video = video[:, 0]
-        return video if n_samples is not None else video[0]
+        c = self._checked(video_length, n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
+                          guidance_rescale, timestep_spacing, cfg_img)
+        frames = preprocess([image], c.size, self.model.device)
+        return self._generate(frames, prompt, [0], [0], False, False, seed, c, segment_axis=False)
 
     @torch.no_grad()
     def refine(self, clip, strength: float, prompt: Union[str, torch.Tensor] = "", keep: Optional[Sequence[int]] = None,
@@ -287,32 +342,15 @@ class ToonCrafterPipeline:
 
         Returns what a one-segment interpolate returns: uint8 [T, size[0], size[1], 3], or float32 [3, T, size[0],
         size[1]] with output="float"; an integer n_samples adds a leading variant axis.  ValueError for a bad clip
-        length, strength, keep, n_samples or output before any work."""
-        T = check_video_length(len(clip))
-        if (isinstance(strength, bool) or not isinstance(strength, (int, float, np.integer, np.floating))
-                or not 0.0 < strength <= 1.0):
-            raise ValueError(f"strength must be a number in (0, 1], got {strength!r}")
-        k = int(strength * steps)
-        if k < 1:
-            raise ValueError(f"strength {strength} x steps {steps} runs no DDIM step (int(strength * steps) < 1)")
-        if keep is not None:
-            keep = list(keep)
-            if any(isinstance(j, bool) or not isinstance(j, (int, np.integer)) or not 0 <= j < T for j in keep):
-                raise ValueError(f"keep must hold frame indices from 0 to {T - 1}, got {keep!r}")
-            if len(set(int(j) for j in keep)) != len(keep):
-                raise ValueError(f"keep lists a frame twice: {keep!r}")
-            keep = sorted(int(j) for j in keep) or None
-        n = 1 if n_samples is None else check_n_samples(n_samples)
-        if segments_per_batch is None:
-            segments_per_batch = default_segments_per_batch(size, T)
-        frames = self._preprocess(clip, size, output)
-        init = dict(frames=frames[1:T - 1], seeds=[seed + 1 + j for j in range(1, T - 1)], k=k, keep=keep)
-        video = self._generate(frames[[0, T - 1]], prompt, [0], [1], True, False, seed, n, segments_per_batch, output,
-                               T, _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img),
-                               init=init)
-        if output == "float":
-            video = video[:, 0]
-        return video if n_samples is not None else video[0]
+        length, strength, keep, n_samples, segments_per_batch or output before any work."""
+        c = self._checked(len(clip), n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
+                          guidance_rescale, timestep_spacing, cfg_img)
+        T = c.T
+        k, keep = check_strength(strength, steps), check_keep(keep, T)
+        frames = preprocess(clip, c.size, self.model.device)
+        start = _Refine(frames[1:T - 1], [seed + 1 + j for j in range(1, T - 1)], k, keep)
+        return self._generate(frames[[0, T - 1]], prompt, [0], [1], True, False, seed, c, segment_axis=False,
+                              refine=start)
 
     @torch.no_grad()
     def interpolate_pairs(self, pairs, prompts: Union[str, Sequence[str], torch.Tensor] = "", n_samples: int = 1,
@@ -331,140 +369,161 @@ class ToonCrafterPipeline:
 
         Returns uint8 [P, n, T, size[0], size[1], 3] on the model's device, every pair's whole clip; with
         output="float", float32 [P, n, 3, T, size[0], size[1]]."""
-        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
-        n = check_n_samples(n_samples)
         P = len(pairs)
         if P < 1 or any(len(p) != 2 for p in pairs):
             raise ValueError("pairs must be a non-empty sequence of (image, image) pairs")
-        if isinstance(prompts, torch.Tensor):
-            if prompts.dim() != 2 or prompts.shape[0] != P:
-                raise ValueError(f"token ids must be [P={P}, 77], got {tuple(prompts.shape)}")
-        elif not isinstance(prompts, str) and len(prompts) != P:
-            raise ValueError(f"{len(prompts)} prompts for {P} pairs")
-        if pairs_per_batch is None:
-            pairs_per_batch = default_pairs_per_batch(size, T, n)
-        elif isinstance(pairs_per_batch, bool) or not isinstance(pairs_per_batch, int) or pairs_per_batch < 1:
-            raise ValueError(f"pairs_per_batch must be an integer >= 1, got {pairs_per_batch!r}")
-        self._check_arguments(size, output)
-        sampling = _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img)
-        self._check_latency(sampling)
-        dev = self.model.device
-        video = (torch.empty(P * n * T, size[0], size[1], 3, dtype=torch.uint8, device=dev) if output == "uint8"
-                 else torch.empty(P * n, 3, T, size[0], size[1], dtype=torch.float32, device=dev))
+        _check_prompts(prompts, P, "pairs")
+        c = self._checked(video_length, n_samples, pairs_per_batch, size, output, steps, cfg_scale, eta, fs,
+                          guidance_rescale, timestep_spacing, cfg_img, pairs=True)
+        n, T = c.n, c.T
+        # pair-major rows: pair i's variant v is row i * n + v, its whole clip (frames 0 .. T-1, no seam)
+        rows = [_Row(i, seed + i + v * VARIANT_SEED_STRIDE, i * n + v, 0, T, (i * n + v) * T)
+                for i in range(P) for v in range(n)]
+        video = self._empty(rows, c)
         mine = self._mine(P)
-        for g0 in range(0, len(mine), pairs_per_batch):
-            group = mine[g0:g0 + pairs_per_batch]
-            frames = preprocess([im for i in group for im in pairs[i]], size, dev)
+        for g0 in range(0, len(mine), c.per_batch):
+            group = mine[g0:g0 + c.per_batch]
+            frames = preprocess([im for i in group for im in pairs[i]], c.size, self.model.device)
             text = prompts if isinstance(prompts, str) else (prompts[group] if isinstance(prompts, torch.Tensor)
                                                              else [prompts[i] for i in group])
-            # pair-major rows: pair i's variant v is video row i * n + v, whole (frames 0 .. T-1, no seam)
-            rows = [(k, seed + i + v * VARIANT_SEED_STRIDE, i * n + v if output == "float" else (0, T, (i * n + v) * T))
-                    for k, i in enumerate(group) for v in range(n)]
+            batch = [r._replace(seg=r.seg - group[0]) for r in rows[group[0] * n:(group[-1] + 1) * n]]
             G = len(group)
             self._render(frames, text, [2 * k for k in range(G)], [2 * k + 1 for k in range(G)], True,
-                         [seed + i + j for i in group for j in (0, 1)], rows, len(rows), video, T, sampling)
-        per_pair = n if output == "float" else n * T
-        self._broadcast(video, P, lambda i0, i1: (i0 * per_pair, i1 * per_pair))
-        return (video.view(P, n, T, size[0], size[1], 3) if output == "uint8"
-                else video.view(P, n, 3, T, size[0], size[1]))
+                         [seed + i + j for i in group for j in (0, 1)], batch, len(batch), video, c)
+        self._broadcast(video, rows, n, c.output)
+        return (video.view(P, n, T, *c.size, 3) if c.output == "uint8" else video.view(P, n, 3, T, *c.size))
 
-    def _check_arguments(self, size, output) -> None:
+    def _checked(self, video_length, n_samples, per_batch, size, output, steps, cfg_scale, eta, fs, guidance_rescale,
+                 timestep_spacing, cfg_img, pairs: bool = False) -> _Call:
+        """The argument checks the public methods share, all before any work; returns the normalised arguments.
+        video_length None: the model's temporal_length.  per_batch: segments_per_batch, or pairs_per_batch with
+        `pairs` (where n_samples must be an integer); None: its default."""
+        T = check_video_length(self.model.temporal_length if video_length is None else video_length)
+        n = check_n_samples(n_samples) if pairs or n_samples is not None else 1
+        if per_batch is not None:
+            per_batch = check_count(per_batch, "pairs_per_batch" if pairs else "segments_per_batch")
+        else:
+            per_batch = default_pairs_per_batch(size, T, n) if pairs else default_segments_per_batch(size, T)
         if output not in ("uint8", "float"):
             raise ValueError(f"output must be 'uint8' or 'float', got {output!r}")
         if size[0] % 16 or size[1] % 16:
             raise ValueError(f"size {tuple(size)} must be a multiple of 16")
         if self.model.model.conditioning_key != "hybrid":
             raise NotImplementedError("image-conditioned synthesis needs the hybrid (concat + cross-attention) model")
-
-    def _preprocess(self, images, size, output) -> torch.Tensor:
-        """Argument checks shared by interpolate and animate, then preprocess() onto the model's device."""
-        self._check_arguments(size, output)
-        return preprocess(images, size, self.model.device)
-
-    def _check_latency(self, sampling) -> None:
-        if not self.latency:
-            return
-        if sampling["cfg_img"] is not None:
+        if self.latency and cfg_img is not None:
             raise NotImplementedError("latency mode splits two guidance branches over a GPU pair; three-way "
                                       "guidance (cfg_img) is not supported")
-        if sampling["cfg_scale"] == 1.0:
+        if self.latency and cfg_scale == 1.0:
             raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
                              "cfg_scale 1.0 has no unconditional branch")
+        return _Call(T, n, per_batch, pairs or n_samples is not None, tuple(size), output, steps, cfg_scale, eta, fs,
+                     guidance_rescale, timestep_spacing, cfg_img)
 
     def _mine(self, n_items: int):
         """The items (rows, pairs) of this rank's block: all of them without a group."""
         return list(range(n_items)) if self.group is None else distributed.shard_clips(n_items, self._block,
                                                                                        self._n_blocks)
 
-    def _broadcast(self, video, n_items: int, span) -> None:
-        """With a group: give every rank the whole `video`, block b's items [i0, i1) being video[span(i0, i1)] of
-        the rank that computed them."""
+    def _empty(self, rows, c: _Call) -> torch.Tensor:
+        """The flattened output that all of the call's `rows` fill."""
+        if c.output == "float":
+            return torch.empty(len(rows), 3, c.T, *c.size, dtype=torch.float32, device=self.model.device)
+        return torch.empty(_span(rows, "uint8")[1], *c.size, 3, dtype=torch.uint8, device=self.model.device)
+
+    def _broadcast(self, video, rows, per_item: int, output: str) -> None:
+        """With a group: give every rank the whole `video`.  The items _mine shards are the groups of `per_item`
+        consecutive `rows` (all of the call's rows); block b's rows write their span of the rank that computed them."""
         if self.group is None:
             return
         blocks = []
         for b in range(self._n_blocks):
-            items = distributed.shard_clips(n_items, b, self._n_blocks)
-            if items:
-                blocks.append((self._owner(b),) + tuple(span(items[0], items[-1] + 1)))
+            items = distributed.shard_clips(len(rows) // per_item, b, self._n_blocks)
+            if items:                               # held by the rank, or pair-rank 0 of the pair, that computed it
+                owner = dist.get_global_rank(self.group, 2 * b if self.latency else b)
+                blocks.append((owner,) + _span(rows[items[0] * per_item:(items[-1] + 1) * per_item], output))
         distributed.broadcast_blocks(video, blocks, self.group)
 
-    def _generate(self, frames, prompts, first, last, interp: bool, loop, seed, n, rows_per_batch, output, T,
-                  sampling, init=None) -> torch.Tensor:
-        """n variants of S = len(first) segments of T frames; segment k runs from keyframe first[k] to keyframe
+    def _generate(self, frames, prompts, first, last, interp: bool, loop, seed, c: _Call, segment_axis: bool = True,
+                  refine: Optional[_Refine] = None) -> torch.Tensor:
+        """c.n variants of S = len(first) segments of c.T frames; segment k runs from keyframe first[k] to keyframe
         last[k] (interp), or animates keyframe first[k] (not interp).  Row r = v * S + k is variant v of segment k.
-        With a group, this rank computes its block of rows and the blocks are then broadcast.  init: see _render.
-        Returns uint8 [n, F, H, W, 3] or float [n, S, 3, T, H, W]."""
-        self._check_latency(sampling)
-        S = len(first)
-        H, W = frames.shape[-2:]
+        With a group, this rank computes its block of rows and the blocks are then broadcast.
+        Returns uint8 [n, F, H, W, 3] or float [n, S, 3, T, H, W], without the variant axis unless c.variant_axis,
+        and without the float segment axis unless segment_axis."""
+        S, T, n = len(first), c.T, c.n
         F = (T - 1) * S + (0 if loop else 1)
-        dev = self.model.device
-        video = (torch.empty(n * F, H, W, 3, dtype=torch.uint8, device=dev) if output == "uint8"
-                 else torch.empty(n * S, 3, T, H, W, dtype=torch.float32, device=dev))
-
-        def window(r):
-            """(f_begin, f_end, out_frame): the frames of row r's segment kept by the seam rule, and where the first
-            of them goes in the flattened [n * F] video (variant v's video starts at frame v * F)."""
+        rows = []
+        for r in range(n * S):
             v, k = divmod(r, S)
             f_begin, f_end = (1 if k else 0), (T - 1 if (loop and k == S - 1) else T)
-            return f_begin, f_end, v * F + (T - 1) * k + f_begin
+            rows.append(_Row(k, seed + k + v * VARIANT_SEED_STRIDE, r, f_begin, f_end, v * F + (T - 1) * k + f_begin))
+        video = self._empty(rows, c)
+        mine = [rows[r] for r in self._mine(len(rows))]
+        if mine:
+            self._render(frames, prompts, first, last, interp, [seed + j for j in range(frames.shape[0])], mine,
+                         c.per_batch, video, c, refine)
+        self._broadcast(video, rows, 1, c.output)
+        if c.output == "uint8":
+            video = video.view(n, F, *c.size, 3)
+        else:
+            video = video.view(n, S, 3, T, *c.size)
+            if not segment_axis:
+                video = video[:, 0]
+        return video if c.variant_axis else video[0]
 
-        def span(r0, r1):                       # rows r0 .. r1-1 write one contiguous range (variant-major order)
-            if output == "float":
-                return r0, r1
-            a, b = window(r0), window(r1 - 1)
-            return a[2], b[2] + b[1] - b[0]
-
-        rows = [(r % S, seed + r % S + (r // S) * VARIANT_SEED_STRIDE, r if output == "float" else window(r))
-                for r in self._mine(n * S)]
-        if rows:
-            self._render(frames, prompts, first, last, interp, [seed + j for j in range(frames.shape[0])], rows,
-                         rows_per_batch, video, T, sampling, init)
-        self._broadcast(video, n * S, span)
-        return video.view(n, F, H, W, 3) if output == "uint8" else video.view(n, S, 3, T, H, W)
-
-    def _render(self, frames, prompts, first, last, interp: bool, key_seeds, rows, rows_per_batch, video, T,
-                sampling, init=None) -> None:
-        """Sample and decode `rows` into their places in `video`.  rows: [(segment k of S = len(first), the seed of
-        its x_T and step noise, its place)], sampled `rows_per_batch` at a time; the place is the row's index in
-        float `video` [R, 3, T, H, W], or (f_begin, f_end, out_frame) of tc_video_u8 for uint8 `video`.
-        key_seeds[j]: the seed of keyframe j's posterior noise.
-
-        init (refine; one segment whose keyframes 0 and 1 are the clip's first and last frames): dict(frames=the
-        preprocessed frames 1 .. T-2, seeds=their posterior-noise seeds, k=DDIM steps to run, keep=None or kept frame
-        indices).  Every row then starts from the clip's latents stochastic_encode'd to DDIM index k - 1 with noise
-        drawn first from the row's generator, and samples the last k steps (with keep: mask / x0 on those frames)."""
+    def _render(self, frames, prompts, first, last, interp: bool, key_seeds, rows, rows_per_batch, video, c: _Call,
+                refine: Optional[_Refine] = None) -> None:
+        """Sample and decode `rows` (consecutive, rows_per_batch per sample() call) into `video`.  Segment k of S =
+        len(first) runs from keyframe first[k] to keyframe last[k] (interp), or animates keyframe first[k]; keyframe
+        j's posterior noise is seeded key_seeds[j].  refine: every row starts from the clip's latents (_refine_start)."""
         m = self.model
-        dev = m.device
-        n_dec = m.en_and_decode_n_samples_a_time or m.temporal_length                # decode_core's chunk
-        ex = runtime.TEST_EXECUTOR
-        K, S = frames.shape[0], len(first)
-        steps, cfg_scale, cfg_img = sampling["steps"], sampling["cfg_scale"], sampling["cfg_img"]
+        T = c.T
+        emb = self._conditioning(frames, prompts, first)
+        post, hidden = m.first_stage_model.encode(frames, return_hidden_states=True)
+        z = _posterior_sample(m, post, key_seeds)                                    # [K, 4, h, w]
+        if interp:
+            c_concat = torch.zeros(len(first), z.shape[1], T, *z.shape[-2:], dtype=z.dtype, device=m.device)
+            c_concat[:, :, 0] = z[first]
+            c_concat[:, :, -1] = z[last]
+        else:
+            c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
+        x0 = None if refine is None else self._clip_latents(z, refine.frames, refine.seeds)   # [1, 4, T, h, w]
 
-        # conditioning: text over the distinct prompts + "", image over each segment's first keyframe + the zero image
-        # (over all S segments whatever the rows are: the towers' batch size stays that of the single-process call,
-        # and the variants of a segment share its conditioning)
-        cond_emb, empty_emb = self._text(prompts, S)
+        sampler = DDIMSampler(m) if c.cfg_img is None else DDIMSamplerMultiCond(m)
+        sampler.latency_group = self._pair
+        decodes = not (self.latency and self._pair_rank)          # in a latency pair, pair-rank 0 decodes
+        dec = m.first_stage_model.decoder_engine() if decodes else None
+        dual_ref = isinstance(m.first_stage_model.decoder, VideoDecoder)
+        for g0 in range(0, len(rows), rows_per_batch):
+            batch = rows[g0:g0 + rows_per_batch]
+            gens = [torch.Generator(device=m.device).manual_seed(r.seed) for r in batch]
+            start = {} if refine is None else self._refine_start(sampler, x0, refine, gens, c)
+            samples = self._sample(sampler, emb, c_concat, [r.seg for r in batch], gens, start, c)
+            if not decodes:
+                continue
+            for row, sample in zip(batch, samples):
+                ref = ([torch.stack([hd[first[row.seg]], hd[last[row.seg]]], 1).unsqueeze(0) for hd in hidden]
+                       if dual_ref else None)
+                self._write_row(dec, video, row, sample, ref, T)
+
+    def _conditioning(self, frames, prompts, first):
+        """(text, unconditional text, image, unconditional image) embeddings of the S = len(first) segments: one text-
+        tower pass over the distinct prompts + "", one image-tower pass over each segment's first keyframe + the zero
+        image.  Over all S segments whatever rows are sampled: the towers' batch size stays that of the single-process
+        call, and the variants of a segment share its conditioning."""
+        m = self.model
+        S = len(first)
+        _check_prompts(prompts, S, "segments")
+        if isinstance(prompts, torch.Tensor):
+            uniq, inv = torch.unique(prompts.long().cpu(), dim=0, return_inverse=True)
+            emb = m.get_learned_conditioning(torch.cat([uniq, clip_tokenize([""], prompts.shape[1])]).to(m.device))
+            cond_emb, empty_emb = emb[inv.to(emb.device)], emb[-1:]
+        else:
+            texts = [prompts] * S if isinstance(prompts, str) else list(prompts)
+            distinct = list(dict.fromkeys(texts + [""]))
+            emb = m.get_learned_conditioning(distinct)
+            idx = torch.tensor([distinct.index(t) for t in texts], device=emb.device)
+            cond_emb, empty_emb = emb[idx], emb[distinct.index("")][None]
         if m.uncond_type == "empty_seq":
             uc_emb = empty_emb.expand_as(cond_emb)
         elif m.uncond_type == "zero_embed":
@@ -473,88 +532,7 @@ class ToonCrafterPipeline:
             raise NotImplementedError(f"uncond_type {m.uncond_type!r}")
         img = torch.cat([frames[first], torch.zeros_like(frames[:1])])
         img_all = m.image_proj_model(m.embedder(img))
-        img_emb, uc_img_emb = img_all[:S], img_all[S:].expand(S, -1, -1)
-
-        # first stage: the K distinct keyframes once; keyframe j's posterior noise from a CPU generator seeded
-        # key_seeds[j]
-        post, hidden = m.first_stage_model.encode(frames, return_hidden_states=True)
-        noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(s))
-                             for s in key_seeds])
-        z = m.get_first_stage_encoding(post, noise=noise)                           # [K, 4, h, w]
-        h, w = z.shape[-2:]
-        if interp:
-            c_concat = torch.zeros(S, z.shape[1], T, h, w, dtype=z.dtype, device=dev)
-            c_concat[:, :, 0] = z[first]
-            c_concat[:, :, -1] = z[last]
-        else:
-            c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
-        if init is not None:
-            x0 = self._clip_latents(z, init["frames"], init["seeds"])                  # [1, 4, T, h, w]
-            mask = None
-            if init["keep"] is not None:
-                mask = torch.zeros(1, 1, T, 1, 1, dtype=torch.float32, device=dev)
-                mask[:, :, init["keep"]] = 1.0
-
-        sampler = DDIMSampler(m) if cfg_img is None else DDIMSamplerMultiCond(m)
-        sampler.latency_group = self._pair
-        decodes = not (self.latency and self._pair_rank)          # in a latency pair, pair-rank 0 decodes
-        dec = m.first_stage_model.decoder_engine() if decodes else None
-        dual_ref = isinstance(m.first_stage_model.decoder, VideoDecoder)
-        keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
-        for g0 in range(0, len(rows), rows_per_batch):
-            batch = rows[g0:g0 + rows_per_batch]
-            seg = [k for k, _, _ in batch]
-            b = len(seg)
-            cc = [c_concat[seg]]
-            cond = {"c_crossattn": [torch.cat([cond_emb[seg], img_emb[seg]], 1)], "c_concat": cc}
-            uc = ({"c_crossattn": [torch.cat([uc_emb[seg], uc_img_emb[seg]], 1)], "c_concat": cc}
-                  if cfg_scale != 1.0 else None)
-            extra = {}
-            if cfg_img is not None:
-                extra = dict(cfg_img=cfg_img, unconditional_conditioning_img_nonetext={
-                    "c_crossattn": [torch.cat([uc_emb[seg], img_emb[seg]], 1)], "c_concat": cc})
-            gens = [torch.Generator(device=dev).manual_seed(s) for _, s, _ in batch]
-            if init is not None:
-                shape = (b, z.shape[1], T, h, w)
-                sampler.make_schedule(steps, sampling["timestep_spacing"], sampling["eta"], verbose=False)
-                x_k = sampler.stochastic_encode(x0.expand(shape), torch.full((b,), init["k"] - 1, device=dev),
-                                                noise=randn_rows(shape, dev, gens))
-                extra = dict(extra, x_T=x_k, t_start=init["k"])
-                if mask is not None:
-                    extra.update(mask=mask, x0=x0.expand(shape).contiguous())
-            samples, _ = sampler.sample(S=steps, conditioning=cond, batch_size=b, shape=[z.shape[1], T, h, w],
-                                        verbose=False, unconditional_guidance_scale=cfg_scale,
-                                        unconditional_conditioning=uc, eta=sampling["eta"],
-                                        fs=torch.tensor([sampling["fs"]] * b, dtype=torch.long, device=dev),
-                                        timestep_spacing=sampling["timestep_spacing"],
-                                        guidance_rescale=sampling["guidance_rescale"], noise_generators=gens, **extra)
-            if not decodes:
-                continue
-            for i, (k, _, place) in enumerate(batch):
-                lat = (1.0 / m.scale_factor * samples[i]).permute(1, 0, 2, 3)          # decode_core order
-                if dual_ref:
-                    ref = [torch.stack([hd[first[k]], hd[last[k]]], 1).unsqueeze(0) for hd in hidden]
-                    y16 = _decode_chunks(dec, lat, n_dec, ref, ex)      # a view of the plan's output for T <= n_dec
-                    y14 = _decode_chunks(dec, lat[keep], n_dec, ref, ex)
-                else:
-                    # A frame-independent decoder turns each latent into the same frame whichever chunk holds it, so
-                    # the reference's T - 2 pass is y16[keep] and the T - 2 decode is skipped.  For T >= 6 the two
-                    # spliced frames (keep[T/2-2], keep[T/2-1] = latents T/2-1, T/2) are the frames already in place:
-                    # no splice at all (tc_video_u8 with x14 = NULL).
-                    y16 = _decode_chunks(dec, lat, n_dec, None, ex)
-                    y14 = None if T >= 6 else y16[keep]
-                if video.dtype == torch.float32:
-                    v = y16.float()
-                    if y14 is not None:
-                        v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
-                    video[place] = v.permute(1, 0, 2, 3)
-                    continue
-                f_begin, f_end, out_frame = place
-                args, kw = (y16, y14, video), dict(f_begin=f_begin, f_end=f_end, out_frame=out_frame)
-                if ex is not None:
-                    ex(ops.video_u8, args, kw)
-                else:
-                    ops.video_u8(*args, **kw)
+        return cond_emb, uc_emb, img_all[:S], img_all[S:].expand(S, -1, -1)
 
     def _clip_latents(self, z_ends, interior, seeds) -> torch.Tensor:
         """[1, 4, T, h, w] latents of a clip: frames 0 and T-1 from z_ends [2, 4, h, w], frames 1 .. T-2 encoded from
@@ -567,12 +545,70 @@ class ToonCrafterPipeline:
         x0[0, :, 0], x0[0, :, T - 1] = z_ends[0], z_ends[1]
         for i in range(0, T - 2, n_enc):
             post = m.first_stage_model.encode(interior[i:i + n_enc])
-            noise = torch.stack([torch.randn(tuple(post.mean.shape[1:]), generator=torch.Generator().manual_seed(s))
-                                 for s in seeds[i:i + n_enc]])
-            x0[0, :, 1 + i:1 + i + post.mean.shape[0]] = m.get_first_stage_encoding(post, noise=noise).transpose(0, 1)
+            x0[0, :, 1 + i:1 + i + post.mean.shape[0]] = _posterior_sample(m, post, seeds[i:i + n_enc]).transpose(0, 1)
         return x0
 
+    def _refine_start(self, sampler, x0, refine: _Refine, gens, c: _Call) -> dict:
+        """sample()'s keywords that start a batch of len(gens) rows from the clip's latents x0, stochastic_encode'd to
+        DDIM index k - 1 with noise drawn first from each row's generator, and run the last k steps (with keep: mask
+        and x0 on the kept frames)."""
+        dev = self.model.device
+        shape = (len(gens),) + tuple(x0.shape[1:])
+        sampler.make_schedule(c.steps, c.timestep_spacing, c.eta, verbose=False)
+        x_k = sampler.stochastic_encode(x0.expand(shape), torch.full((len(gens),), refine.k - 1, device=dev),
+                                        noise=randn_rows(shape, dev, gens))
+        start = dict(x_T=x_k, t_start=refine.k)
+        if refine.keep is not None:
+            mask = torch.zeros(1, 1, c.T, 1, 1, dtype=torch.float32, device=dev)
+            mask[:, :, refine.keep] = 1.0
+            start.update(mask=mask, x0=x0.expand(shape).contiguous())
+        return start
 
-def _sampling(steps, cfg_scale, eta, fs, guidance_rescale, timestep_spacing, cfg_img) -> dict:
-    return dict(steps=steps, cfg_scale=cfg_scale, eta=eta, fs=fs, guidance_rescale=guidance_rescale,
-                timestep_spacing=timestep_spacing, cfg_img=cfg_img)
+    def _sample(self, sampler, emb, c_concat, seg, gens, start: dict, c: _Call) -> torch.Tensor:
+        cond_emb, uc_emb, img_emb, uc_img_emb = emb
+        b = len(seg)
+        cc = [c_concat[seg]]
+        cond = {"c_crossattn": [torch.cat([cond_emb[seg], img_emb[seg]], 1)], "c_concat": cc}
+        uc = ({"c_crossattn": [torch.cat([uc_emb[seg], uc_img_emb[seg]], 1)], "c_concat": cc}
+              if c.cfg_scale != 1.0 else None)
+        if c.cfg_img is not None:
+            start = dict(start, cfg_img=c.cfg_img, unconditional_conditioning_img_nonetext={
+                "c_crossattn": [torch.cat([uc_emb[seg], img_emb[seg]], 1)], "c_concat": cc})
+        samples, _ = sampler.sample(S=c.steps, conditioning=cond, batch_size=b, shape=list(c_concat.shape[1:]),
+                                    verbose=False, unconditional_guidance_scale=c.cfg_scale,
+                                    unconditional_conditioning=uc, eta=c.eta,
+                                    fs=torch.tensor([c.fs] * b, dtype=torch.long, device=self.model.device),
+                                    timestep_spacing=c.timestep_spacing, guidance_rescale=c.guidance_rescale,
+                                    noise_generators=gens, **start)
+        return samples
+
+    def _write_row(self, dec, video, row: _Row, sample, ref, T: int) -> None:
+        """Decode one row's latents [4, T, h, w] and write it into `video` at its place: the spliced clip in float
+        output, its seam-rule frames through tc_video_u8 in uint8 output.  ref: the dual-reference decoder's maps, None
+        with a plain first stage."""
+        m = self.model
+        n_dec = m.en_and_decode_n_samples_a_time or m.temporal_length                # decode_core's chunk
+        ex = runtime.TEST_EXECUTOR
+        keep = [t for t in range(T) if t not in (1, T - 2)]                           # inference.py:264-267
+        lat = (1.0 / m.scale_factor * sample).permute(1, 0, 2, 3)                    # decode_core order
+        if ref is not None:
+            y16 = _decode_chunks(dec, lat, n_dec, ref, ex)          # a view of the plan's output for T <= n_dec
+            y14 = _decode_chunks(dec, lat[keep], n_dec, ref, ex)
+        else:
+            # A frame-independent decoder turns each latent into the same frame whichever chunk holds it, so the
+            # reference's T - 2 pass is y16[keep] and the T - 2 decode is skipped.  For T >= 6 the two spliced frames
+            # (keep[T/2-2], keep[T/2-1] = latents T/2-1, T/2) are the frames already in place: no splice at all
+            # (tc_video_u8 with x14 = NULL).
+            y16 = _decode_chunks(dec, lat, n_dec, None, ex)
+            y14 = None if T >= 6 else y16[keep]
+        if video.dtype == torch.float32:
+            v = y16.float()
+            if y14 is not None:
+                v[T // 2 - 1:T // 2 + 1] = y14[T // 2 - 2:T // 2].float()
+            video[row.index] = v.permute(1, 0, 2, 3)
+            return
+        args, kw = (y16, y14, video), dict(f_begin=row.f_begin, f_end=row.f_end, out_frame=row.out_frame)
+        if ex is not None:
+            ex(ops.video_u8, args, kw)
+        else:
+            ops.video_u8(*args, **kw)
