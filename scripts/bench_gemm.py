@@ -8,7 +8,7 @@ collected with its launch count per program, then one call of each is replayed o
 operands of the recorded shapes and strides.  Each shape is timed with CUDA events around replays of a CUDA graph of
 back-to-back launches, at least --min-ms of GPU time per shape.
 
-    python scripts/bench_gemm.py --out DIR [--min-ms 100] [--sweep] [--top 15]
+    python scripts/bench_gemm.py --out DIR [--min-ms 100] [--sweep] [--top 15] [--fixed-cost [--fixed-cost-shape MxNxK]]
 
 Reports per shape: microseconds per launch, TFLOP/s, launches per program and the (block_n, k-slices, stages) the
 library chose; per program the launch-weighted GEMM time and its TFLOP/s.  --sweep also times the --top shapes by
@@ -18,6 +18,10 @@ limit and SM clocks (query-only nvidia-smi) are recorded with the numbers.  Writ
 Every shape whose epilogue reads a residual or a per-sample bias (bias2) is timed a second time without those operands,
 at the block_n and k-slices of the recorded call, so both runs use the same tiling.  The difference is what reading
 them costs; it is reported per shape ("operand_us") and summed over a clip ("epilogue_operands").
+
+--fixed-cost measures what a tile costs besides its k-blocks, for 1x1 shapes whose tiles have only a few k-blocks: the
+same M, N and epilogue timed at K = 64 .. 640, at the recorded block_n and one k-slice, fitted as
+time = waves x (c0 + c1 x k-blocks).  c0 is reported in microseconds and in SM cycles at the sampled clock ("fixed_cost").
 """
 from __future__ import annotations
 
@@ -191,12 +195,68 @@ def sweep_options(kw, n_cols):
     return [(bn, cap) for bn in bns for cap in caps]
 
 
+def m_tiles(out_dims):
+    """Output tiles along M: the (TW, TH, TN) box of <= 128 output pixels with the fewest tiles (tc_conv_gemm's search)."""
+    N, H, W = out_dims
+    best = None
+    for tw in range(1, min(W, 128) + 1):
+        for th in range(1, min(128 // tw, H) + 1):
+            tn = min(128 // (tw * th), N)
+            t = -(-W // tw) * -(-H // th) * -(-N // tn)
+            best = t if best is None else min(best, t)
+    return best
+
+
+def fixed_cost(call, block_n, dev, seed, min_ms, kblocks=range(1, 11)):
+    """Fixed per-tile cost of one 1x1 (linear) shape: the same M, N and epilogue at K = 64 k, k = kblocks, one k-slice,
+    the given block_n; least-squares fit of  time = waves x (c0 + c1 k)  (waves = tiles / SMs, rounded up).  c0 is
+    what a tile costs besides its k-blocks: launch share, pipeline fill, epilogue and output stores."""
+    import numpy as np
+    from tooncrafter_b200 import _lib, ops
+    lib = _lib.load()
+    a, kw = materialize(call, dev, seed)
+    a_dims, out_dims, n_cols, w = a[1], a[6], a[7], a[3]
+    g = torch.Generator(device=dev).manual_seed(seed)
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    tiles = m_tiles(out_dims) * -(-n_cols // block_n)
+    waves = -(-tiles // sms)
+    pts = []
+    lib.tc_debug_set_gemm_mode(1 << 8)                 # one k-slice
+    try:
+        for k in kblocks:
+            C = 64 * k
+            N, H, W = a_dims[0], a_dims[1], a_dims[2]
+            x = torch.randn(N * H * W * C, generator=g, device=dev).mul_(0.25).half()
+            wk = torch.randn(w.shape[0], C, generator=g, device=dev).mul_(C ** -0.5).half()
+            args = (x, (N, H, W, C), (H * W * C, W * C, C), wk) + tuple(a[4:])
+            kwk = dict(kw, block_n=block_n, a_offset=0)
+            fn = lambda: ops.conv_gemm(*args, **kwk)
+            us, _ = time_call(fn, min_ms)
+            cfg = ops.last_gemm_config()
+            assert (cfg["block_n"], cfg["ksplit"]) == (block_n, 1), cfg
+            pts.append(dict(kblocks=k, us=round(us, 2)))
+            del x, wk
+    finally:
+        lib.tc_debug_set_gemm_mode(0)
+    ks = np.array([p["kblocks"] for p in pts], dtype=np.float64)
+    per_wave = np.array([p["us"] for p in pts]) / waves
+    c1, c0 = np.polyfit(ks, per_wave, 1)
+    resid = per_wave - (c0 + c1 * ks)
+    return dict(block_n=block_n, tiles=tiles, waves=waves, points=pts, c0_us=round(float(c0), 3),
+                c1_us_per_kblock=round(float(c1), 3), fit_rms_us=round(float(np.sqrt((resid ** 2).mean())), 3))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", required=True, help="output directory (bench_gemm.json)")
     ap.add_argument("--min-ms", type=float, default=100.0, help="GPU time per timed shape (and per sweep point)")
     ap.add_argument("--sweep", action="store_true", help="also time the --top shapes under every block_n / k-slice cap")
     ap.add_argument("--top", type=int, default=15)
+    ap.add_argument("--fixed-cost", action="store_true",
+                    help="also fit the fixed per-tile cost c0 of the clip's 1x1 GEGLU shapes with K <= 640 and of every "
+                         "--fixed-cost-shape (K = 64 .. 640, the recorded block_n, one k-slice)")
+    ap.add_argument("--fixed-cost-shape", action="append", default=None, metavar="MxNxK",
+                    help="1x1 shape for --fixed-cost (repeatable; default 81920x960x320)")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_gemm.py measures the GPU; no CUDA device found")
@@ -256,6 +316,16 @@ def main():
                              | ({"chosen_over_best": row["chosen_over_best"]} if "sweep" in row else {})), flush=True)
             del a, kw
             torch.cuda.empty_cache()
+        if args.fixed_cost:
+            extra = {tuple(int(v) for v in x.split("x")) for x in (args.fixed_cost_shape or ["81920x960x320"])}
+            for r in rows:
+                k = order[r["rank"]]
+                if r["taps"] != 1 or not (r["epilogue"]["geglu"] and r["K"] <= 640 or (r["M"], r["N"], r["K"]) in extra):
+                    continue
+                r["fixed_cost"] = fixed_cost(shapes[k]["call"], r["config"]["block_n"], dev, r["rank"], args.min_ms / 2)
+                print(json.dumps({x: r[x] for x in ("rank", "M", "N", "K", "us")} | {"fixed_cost": r["fixed_cost"]}),
+                      flush=True)
+                torch.cuda.empty_cache()
     finally:
         lib.tc_debug_set_gemm_mode(0)
         clk = clocks.stop()
@@ -280,11 +350,18 @@ def main():
                clip=dict(gemm_ms=round(clip_ms, 1), tflop=round(clip_flop / 1e12, 1),
                          tflops=round(clip_flop / clip_ms / 1e9, 1)),
                epilogue_operands=epi_ops, shapes=rows)
+    fits = [r for r in rows if "fixed_cost" in r]
+    if fits:
+        mhz = clk.get("sm_mhz_median")
+        out["fixed_cost"] = [dict(M=r["M"], N=r["N"], K=r["K"], epilogue=r["epilogue"], us=r["us"],
+                                  c0_us=r["fixed_cost"]["c0_us"], c1_us_per_kblock=r["fixed_cost"]["c1_us_per_kblock"],
+                                  c0_sm_cycles=round(r["fixed_cost"]["c0_us"] * mhz) if mhz else None,
+                                  block_n=r["fixed_cost"]["block_n"], waves=r["fixed_cost"]["waves"]) for r in fits]
     od = Path(args.out)
     od.mkdir(parents=True, exist_ok=True)
     (od / "bench_gemm.json").write_text(json.dumps(out, indent=1))
     print(json.dumps(dict(gpu=info, clocks_during_run=clk, programs=programs, clip=out["clip"],
-                           epilogue_operands=epi_ops)), flush=True)
+                           epilogue_operands=epi_ops) | ({"fixed_cost": out["fixed_cost"]} if fits else {})), flush=True)
     return 0
 
 

@@ -16,14 +16,17 @@
 //                                  N = BNp (BN rounded up to 32), so A is read from shared memory once per step for all
 //                                  columns; fp32 accumulators in registers, one k-block in flight behind the one being
 //                                  issued.  The k-loop makes no function call (see tc::mbar_wait), which would make
-//                                  ptxas serialise the wgmmas.  After the last k-block the accumulators go to shared
-//                                  memory (the drained operand ring is reused as an fp32 staging tile), and the same
-//                                  256 threads run the epilogue with one output row per thread and two column groups:
-//                                  folded LayerNorm / bias / timestep embedding / scale / residual or GEGLU -> fp16 ->
-//                                  16-byte stores; optional per-row {sum, sumsq} of the outputs for the consumer's
-//                                  LayerNorm fold.
-//   split-K (few output tiles, long K loops): every slice parks its fp32 tile in a workspace, takes a ticket, and the
-//   last slice to arrive sums all slices in slice order (deterministic) and runs the epilogue.
+//                                  ptxas serialise the wgmmas.  After the last k-block the same 256 threads run the
+//                                  epilogue on the accumulator registers, in their fragment layout: folded LayerNorm /
+//                                  bias / timestep embedding / scale / residual (ldmatrix from its boxes) or GEGLU ->
+//                                  fp16 -> stmatrix into an output tile in the drained operand ring, laid out as the
+//                                  swizzled boxes of an output tensor map -> TMA stores, which clip the rows and columns
+//                                  past the output extent (TMA writes whole 16-byte chunks, so the last n % 8 columns
+//                                  of an n-column output are stored by one thread per row).  Optional per-row {sum, sumsq} of the stored fp16 outputs
+//                                  (for the consumer's LayerNorm fold) are read back from that tile, one row per thread.
+//   split-K (few output tiles, long K loops): every slice parks its fp32 accumulators in a workspace, takes a ticket,
+//   and the last slice to arrive sums all slices in slice order (deterministic) into its registers and runs the
+//   epilogue.
 //
 // Algorithmic flops = 2 * M * n_cols * taps * C.
 #include <stdlib.h>
@@ -46,6 +49,10 @@ struct alignas(64) GemmKParams {
     CUtensorMap tmA;
     CUtensorMap tmB;
     CUtensorMap tmR;                // residual [oN][oH][oW][n_cols] (row stride ldr), boxes of 32 columns
+    CUtensorMap tmO;                // output [oN][oH][oW][out_tma_cols] (row stride ldc), boxes of 2^out_box_lg columns
+    int out_box_lg;                 // 5: 32-column boxes, 64B-swizzled; 4: 16-column boxes, 32B-swizzled
+    int out_tma_cols;               // output columns stored by TMA: out_cols rounded down to 8 (0: no output map)
+    int out_cols;                   // output columns (GEGLU: n_cols / 2); the last out_cols % 8 are stored by threads
     int res_boxes;                  // residual boxes per tile (ceil(BN / 32)), 0 without a residual
     uint32_t res_bytes;             // residual bytes delivered per tile
     uint32_t res_smem;              // shared-memory region of the residual boxes (res_boxes x 8 KiB)
@@ -67,7 +74,7 @@ struct alignas(64) GemmKParams {
     int stages;
     uint32_t a_bytes;               // bytes delivered per A box
     uint32_t b_bytes;               // bytes delivered per B box (BNp rows of 128 bytes)
-    uint32_t ring_bytes;            // operand ring (reused as the fp32 accumulator staging tile)
+    uint32_t ring_bytes;            // operand ring (reused as the fp16 output tile)
     __half* out;
     long long ldc;
     const float* bias;
@@ -105,12 +112,40 @@ __device__ __forceinline__ long long tile_bias2_first(const GemmKParams& p, int 
     return m0 / p.bias2_rows_per;
 }
 
+// Byte offset of 16-byte chunk `chunk` (tile columns 8 chunk .. 8 chunk + 7) of tile row `row` in a tile held as TMA
+// boxes of 2^lg columns (lg = 4 or 5), each [128 rows][2^(lg+1) bytes] with the swizzle of that row width (32B or 64B):
+// chunk q of a row sits at q ^ (bits 7.. of the row's offset).  The eight rows of one 8x8 ldmatrix / stmatrix matrix then
+// fall on eight different 16-byte bank groups.
+__device__ __forceinline__ uint32_t swz_offset(int lg, int row, int chunk) {
+    const int per_row = 1 << (lg - 3);
+    const uint32_t row_off = (uint32_t)row << (lg + 1);
+    const uint32_t q = (uint32_t)(chunk & (per_row - 1)) ^ ((row_off >> 7) & (uint32_t)(per_row - 1));
+    return (uint32_t)(chunk >> (lg - 3)) * (uint32_t)(kBlockM << (lg + 1)) + row_off + (q << 4);
+}
+
+// four 8x8 fp16 matrices; lanes 8 i .. 8 i + 7 give the row addresses of matrix i, register i holds this lane's pair
+// (row lane / 4, columns 2 (lane % 4) + {0, 1}) of matrix i: the wgmma accumulator fragment order
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t (&r)[4]) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+                 : "r"(addr)
+                 : "memory");
+}
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+    asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]),
+                 "r"(r[2]), "r"(r[3])
+                 : "memory");
+}
+
+__device__ __forceinline__ float2 h2_to_f2(uint32_t u) {
+    return __half22float2(*reinterpret_cast<const __half2*>(&u));
+}
+
 // kNJ = BNp / 32 (BNp = BN rounded up to 32): the wgmma is m64n(32 kNJ)k16
 template <int kNJ>
 __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_constant__ GemmKParams p) {
     tc::pdl_launch_dependents();   // the successor's prologue may overlap this kernel; it blocks in its own pdl_wait
     constexpr int kBNp = kNJ * 32;
-    constexpr int kLds = kBNp + 4;  // staging row stride in floats (rows 4 banks apart)
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
@@ -118,7 +153,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     const int BN = p.BN;
     uint8_t* sA = smem;
     uint8_t* sB = smem + (size_t)S * kAStageBytes;
-    float* stg = reinterpret_cast<float*>(smem);   // [128][kLds] fp32 accumulators, after the ring has drained
+    uint8_t* s_out = smem;                         // fp16 output tile (TMA store boxes), after the ring has drained
     uint8_t* s_res = smem + p.ring_bytes;          // residual boxes: [res_boxes][128 rows][64 B], 64B-swizzled
     __half* s_b2 = reinterpret_cast<__half*>(s_res + p.res_smem);   // [bias2_rows_max][BN]
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(s_res + p.res_smem + p.b2_smem);
@@ -134,6 +169,7 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
     if (tid == 0) {
         tc::tma_prefetch_desc(&p.tmA);
         tc::tma_prefetch_desc(&p.tmB);
+        if (p.out_tma_cols) tc::tma_prefetch_desc(&p.tmO);
         if (p.res_boxes) tc::tma_prefetch_desc(&p.tmR);
         for (int s = 0; s < S; ++s) {
             tc::mbar_init(&full_bar[s], 1);
@@ -286,32 +322,22 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
         }
         tc::wgmma_wait<0>();
     }
-    // every MMA of both warpgroups has retired (the operand ring becomes the accumulator staging tile), and warps 1-3
-    // have stored the LayerNorm statistics and bias2 rows
+    // every MMA of both warpgroups has retired (the operand ring becomes the fp16 output tile), and warps 1-3 have
+    // stored the LayerNorm statistics and bias2 rows
     asm volatile("bar.sync 2, 352;" ::: "memory");
     // every k-slice waits, so that no CTA exits with its residual load in flight
     if (p.res_boxes) tc::mbar_wait(res_bar, 0);
-    {
-        const int r0 = wg * 64 + warp * 16 + (lane >> 2);
-#pragma unroll
-        for (int j = 0; j < kNJ; ++j)
-#pragma unroll
-            for (int i = 0; i < 16; i += 2) {
-                const int r = r0 + 8 * ((i >> 1) & 1);
-                const int c = j * 32 + 8 * (i >> 2) + 2 * (lane & 3);
-                *reinterpret_cast<float2*>(stg + r * kLds + c) = make_float2(acc[16 * j + i], acc[16 * j + i + 1]);
-            }
-    }
-    asm volatile("bar.sync 1, 256;" ::: "memory");
 
     if (p.ksplit > 1) {
-        // park this slice, take a ticket; only the last slice of the tile goes on and sums the slices in slice order
-        float* ws_tile = p.ws_partial + (long long)tile * p.ksplit * kBlockM * kBNp;
-        float4* wslice = reinterpret_cast<float4*>(ws_tile + (long long)ks * kBlockM * kBNp);
-        for (int i = et; i < kBlockM * kBNp / 4; i += kEpiThreads) {
-            const int r = i / (kBNp / 4), c4 = i - r * (kBNp / 4);
-            __stcg(wslice + i, *reinterpret_cast<const float4*>(stg + r * kLds + 4 * c4));
-        }
+        // park this slice's accumulators (float4 v of thread et at v * 256 + et: a warp's store writes 512 contiguous
+        // bytes), take a ticket; only the last slice of the tile goes on and sums the slices in slice order into acc
+        constexpr int kSliceV4 = kBlockM * kBNp / 4;   // = 4 kNJ float4 per thread
+        float4* ws_tile = reinterpret_cast<float4*>(p.ws_partial) + (long long)tile * p.ksplit * kSliceV4;
+        float4* wslice = ws_tile + (long long)ks * kSliceV4;
+#pragma unroll
+        for (int v = 0; v < 4 * kNJ; ++v)
+            __stcg(wslice + v * kEpiThreads + et,
+                   make_float4(acc[4 * v], acc[4 * v + 1], acc[4 * v + 2], acc[4 * v + 3]));
         __threadfence();
         asm volatile("bar.sync 1, 256;" ::: "memory");
         if (et == 0) {
@@ -324,98 +350,144 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
         asm volatile("bar.sync 1, 256;" ::: "memory");
         if (s_flag[0] == 0) return;
         __threadfence();
-        for (int i = et; i < kBlockM * kBNp / 4; i += kEpiThreads) {
-            const int r = i / (kBNp / 4), c4 = i - r * (kBNp / 4);
-            float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-            for (int sl = 0; sl < p.ksplit; ++sl) {
-                const float4 u = __ldcg(reinterpret_cast<const float4*>(ws_tile + (long long)sl * kBlockM * kBNp) + i);
-                s.x += u.x; s.y += u.y; s.z += u.z; s.w += u.w;
+#pragma unroll
+        for (int i = 0; i < 16 * kNJ; ++i) acc[i] = 0.f;
+        for (int sl = 0; sl < p.ksplit; ++sl) {
+            const float4* src = ws_tile + (long long)sl * kSliceV4 + et;
+#pragma unroll
+            for (int v = 0; v < 4 * kNJ; ++v) {
+                const float4 u = __ldcg(src + v * kEpiThreads);
+                acc[4 * v] += u.x;
+                acc[4 * v + 1] += u.y;
+                acc[4 * v + 2] += u.z;
+                acc[4 * v + 3] += u.w;
             }
-            *reinterpret_cast<float4*>(stg + r * kLds + 4 * c4) = s;
         }
-        asm volatile("bar.sync 1, 256;" ::: "memory");
     }
 
-    // ---------------------------------------------------------------------- epilogue: one row per thread, 2 column groups
-    const int row = et & 127;
-    const int cg = et >> 7;
-    long long m;
-    const bool row_ok = tile_row(p, tx, ty, tn, row, m);
+    // ---------------------------------------------------------------------- epilogue, in the accumulators' layout
+    // Thread (warp, lane) of warpgroup wg holds rows rb and rb + 8 (rb = 64 wg + 16 warp + lane / 4).  Accumulator
+    // 8 t + 2 k + e is row rb + 8 (k & 1), column 16 t + 8 (k >> 1) + 2 (lane % 4) + e: per 16-column group t, its four
+    // register pairs are this lane's parts of the four 8x8 matrices (k & 1, k >> 1) of one ldmatrix / stmatrix .x4.
     const bool geglu = p.geglu != 0;
     const int width = geglu ? (BN >> 1) : BN;                   // output columns per tile
-    const int split = ((width / 16 + 1) / 2) * 16;              // group 0: [0, split), group 1: [split, width)
-    const int c_begin = cg == 0 ? 0 : split;
-    const int c_end = cg == 0 ? split : width;
-    const int out_cols = geglu ? (p.n_cols >> 1) : p.n_cols;
     const int col0 = nt * width;                                // first output column of the tile
-
-    float mean = 0.f, rstd = 1.f;
-    if (p.ln_stats) {
-        const float2 st = s_ln[row];
-        mean = st.x;
-        rstd = st.y;
+    const int lg = p.out_box_lg;
+    const int rb = wg * 64 + warp * 16 + (lane >> 2);
+    const int cl = 2 * (lane & 3);
+    // row and 16-byte column chunk (within the group) this lane addresses for ldmatrix / stmatrix: matrix lane / 8
+    const int mrow = wg * 64 + warp * 16 + ((lane >> 3) & 1) * 8 + (lane & 7);
+    const int mchunk = lane >> 4;
+    float mean[2] = {0.f, 0.f}, rstd[2] = {1.f, 1.f};
+    const __half* b2row[2] = {s_b2, s_b2};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int r = rb + 8 * h;
+        if (p.ln_stats) {
+            const float2 st = s_ln[r];
+            mean[h] = st.x;
+            rstd[h] = st.y;
+        }
+        long long m;
+        if (p.bias2 && tile_row(p, tx, ty, tn, r, m))   // rows past the output extent are computed but not stored
+            b2row[h] = s_b2 + (p.b2_per_row ? r : m / p.bias2_rows_per - tile_bias2_first(p, tx, ty, tn)) * BN;
     }
-    const float* srow = stg + row * kLds;
-    const __half* b2row = (p.bias2 && row_ok)
-                              ? s_b2 + (p.b2_per_row ? row : m / p.bias2_rows_per - tile_bias2_first(p, tx, ty, tn)) * BN
-                              : nullptr;
-    // residual: 16-byte chunk q of a 64-byte box row sits at chunk q ^ ((row >> 1) & 3) (CU_TENSOR_MAP_SWIZZLE_64B)
-    const uint8_t* rrow = s_res + row * (kResBoxCols * 2);
-    const int rswz = (row >> 1) & 3;
-    __half* orow = p.out + m * p.ldc + col0;
-    float rs_sum = 0.f, rs_sq = 0.f;
-    if (row_ok) {
-        for (int c = c_begin; c < c_end; c += 8) {
-            const int nvalid = min(8, out_cols - (col0 + c));
-            if (nvalid <= 0) break;
-            float v[8];
-            if (!geglu) {
+    // the tile row this thread reads back once the stores are issued (partial last chunk, row statistics)
+    const int row = et & 127;
+    long long m;
+    const bool row_ok = tile_row(p, tx, ty, tn, row, m);
+    const uint32_t out_u32 = tc::smem_u32(s_out), res_u32 = tc::smem_u32(s_res);
+    if (!geglu) {
 #pragma unroll
-                for (int i = 0; i < 8; ++i) v[i] = rstd * (srow[c + i] - mean * s_u[c + i]) + s_bias[c + i];
-                if (b2row) {
-                    const uint4 u = *reinterpret_cast<const uint4*>(b2row + c);
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
+        for (int t = 0; t < 2 * kNJ; ++t) {
+            if (16 * t >= width) break;
+            uint32_t res[4];
+            if (p.res_boxes) ldmatrix_x4(res_u32 + swz_offset(5, mrow, 2 * t + mchunk), res);
+            uint32_t packed[4];
 #pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float2 f = __half22float2(h2[i]);
-                        v[2 * i] += f.x;
-                        v[2 * i + 1] += f.y;
-                    }
+            for (int k = 0; k < 4; ++k) {
+                const int h = k & 1, c = 16 * t + 8 * (k >> 1) + cl;
+                const float2 u = *reinterpret_cast<const float2*>(s_u + c);
+                const float2 b = *reinterpret_cast<const float2*>(s_bias + c);
+                float v0 = rstd[h] * (acc[8 * t + 2 * k] - mean[h] * u.x) + b.x;
+                float v1 = rstd[h] * (acc[8 * t + 2 * k + 1] - mean[h] * u.y) + b.y;
+                if (p.bias2) {
+                    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(b2row[h] + c));
+                    v0 += f.x;
+                    v1 += f.y;
                 }
                 if (p.acc_scale != 1.0f) {
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) v[i] *= p.acc_scale;
+                    v0 *= p.acc_scale;
+                    v1 *= p.acc_scale;
                 }
                 if (p.res_boxes) {
-                    const uint4 u = *reinterpret_cast<const uint4*>(
-                        rrow + (c / kResBoxCols) * kResBoxBytes + ((((c >> 3) & 3) ^ rswz) << 4));
-                    const __half2* h2 = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-                    for (int i = 0; i < 4; ++i) {
-                        const float2 f = __half22float2(h2[i]);
-                        v[2 * i] += f.x;
-                        v[2 * i + 1] += f.y;
-                    }
+                    const float2 f = h2_to_f2(res[k]);
+                    v0 += f.x;
+                    v1 += f.y;
                 }
-            } else {
-                // weight rows of this N tile are [value half (BN/2) | gate half (BN/2)]
-                const int g = c + width;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const float a = rstd * (srow[c + i] - mean * s_u[c + i]) + s_bias[c + i];
-                    const float xg = rstd * (srow[g + i] - mean * s_u[g + i]) + s_bias[g + i];
-                    v[i] = a * tc::gelu_erf_f(xg);
-                }
+                packed[k] = pack_h2(v0, v1);
             }
-            if (nvalid == 8) {
-                uint4 u;
-                u.x = pack_h2(v[0], v[1]);
-                u.y = pack_h2(v[2], v[3]);
-                u.z = pack_h2(v[4], v[5]);
-                u.w = pack_h2(v[6], v[7]);
-                *reinterpret_cast<uint4*>(orow + c) = u;
-                if (p.row_stats) {
-                    // statistics of the values the consumer will read: the fp16-rounded outputs
+            stmatrix_x4(out_u32 + swz_offset(lg, mrow, 2 * t + mchunk), packed);
+        }
+    } else {
+        // weight rows of this N tile are [value half | gate half], BN = 32 kNJ: gate column c + width is accumulator
+        // 8 (t + kNJ) + 2 k + e of the same thread
+#pragma unroll
+        for (int t = 0; t < kNJ; ++t) {
+            uint32_t packed[4];
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                const int h = k & 1, c = 16 * t + 8 * (k >> 1) + cl, g = c + 16 * kNJ;
+                float v[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const float a = rstd[h] * (acc[8 * t + 2 * k + e] - mean[h] * s_u[c + e]) + s_bias[c + e];
+                    const float xg =
+                        rstd[h] * (acc[8 * (t + kNJ) + 2 * k + e] - mean[h] * s_u[g + e]) + s_bias[g + e];
+                    v[e] = a * tc::gelu_erf_f(xg);
+                }
+                packed[k] = pack_h2(v[0], v[1]);
+            }
+            stmatrix_x4(out_u32 + swz_offset(lg, mrow, 2 * t + mchunk), packed);
+        }
+    }
+    // the tile leaves as TMA boxes of 2^lg columns over the output's (TW, TH, TN) box; TMA drops the rows and columns
+    // past the output extent.  It writes whole 16-byte chunks, so the last out_cols % 8 columns (a partial chunk) are
+    // not part of the output map: one thread per row stores them
+    tc::fence_proxy_async_smem();
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (et == 0 && p.out_tma_cols > col0) {
+        for (int b = 0; b < (width >> lg); ++b)
+            tc::tma_store_4d(s_out + b * (kBlockM << (lg + 1)), &p.tmO, col0 + (b << lg), tx * p.TW, ty * p.TH,
+                             tn * p.TN);
+        tc::bulk_commit_group();
+    }
+    {
+        const int tail = p.out_tma_cols - col0;   // tile column of the partial chunk
+        if (p.out_cols > p.out_tma_cols && tail >= 0 && tail < width && et >= 128) {
+            if (row_ok) {
+                const uint4 u = *reinterpret_cast<const uint4*>(s_out + swz_offset(lg, row, tail >> 3));
+                const __half* hv = reinterpret_cast<const __half*>(&u);
+                __half* dst = p.out + m * p.ldc + p.out_tma_cols;
+#pragma unroll
+                for (int i = 0; i < 7; ++i)
+                    if (i < p.out_cols - p.out_tma_cols) dst[i] = hv[i];
+            }
+        }
+    }
+    if (p.row_stats) {
+        // per-row {sum, sumsq} of the stored fp16 outputs, read back from the tile: one row per thread and two column
+        // groups, summed in column order; column group 1 hands its partials to the thread of group 0 that owns the row
+        const int cg = et >> 7;
+        const int split = ((width / 16 + 1) / 2) * 16;          // group 0: [0, split), group 1: [split, width)
+        const int c_end = cg == 0 ? split : width;
+        float rs_sum = 0.f, rs_sq = 0.f;
+        if (row_ok) {
+            for (int c = cg == 0 ? 0 : split; c < c_end; c += 8) {
+                const int nvalid = min(8, p.n_cols - (col0 + c));
+                if (nvalid <= 0) break;
+                const uint4 u = *reinterpret_cast<const uint4*>(s_out + swz_offset(lg, row, c >> 3));
+                if (nvalid == 8) {
                     const __half2* h2 = reinterpret_cast<const __half2*>(&u);
 #pragma unroll
                     for (int i = 0; i < 4; ++i) {
@@ -423,20 +495,19 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
                         rs_sum += f.x + f.y;
                         rs_sq = fmaf(f.x, f.x, fmaf(f.y, f.y, rs_sq));
                     }
-                }
-            } else {
-                for (int i = 0; i < nvalid; ++i) {
-                    const __half h = __float2half_rn(v[i]);
-                    orow[c + i] = h;
-                    const float f = __half2float(h);
-                    rs_sum += f;
-                    rs_sq = fmaf(f, f, rs_sq);
+                } else {
+                    const __half* hv = reinterpret_cast<const __half*>(&u);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        if (i < nvalid) {
+                            const float f = __half2float(hv[i]);
+                            rs_sum += f;
+                            rs_sq = fmaf(f, f, rs_sq);
+                        }
+                    }
                 }
             }
         }
-    }
-    if (p.row_stats) {
-        // one slot per N tile: column group 1 hands its partials to the thread of group 0 that owns the same row
         if (cg == 1) s_rs[row] = make_float2(rs_sum, rs_sq);
         asm volatile("bar.sync 1, 256;" ::: "memory");
         if (cg == 0 && row_ok) {
@@ -444,6 +515,9 @@ __global__ void __launch_bounds__(kThreads, 1) tc_gemm_kernel(const __grid_const
             p.row_stats[m * p.row_stats_slots + nt] = make_float2(rs_sum + o.x, rs_sq + o.y);
         }
     }
+    // the stores have completed (not only read the tile) before the CTA exits: a dependent kernel's
+    // griddepcontrol.wait then sees the output
+    if (et == 0) tc::bulk_wait_group<0>();
 }
 
 // Tile-shape heuristic: pick (block_n, k-slices) minimising   waves x per-tile cycles   with a small model of one
@@ -687,10 +761,28 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
         p.b2_smem = (uint32_t)((p.b2_per_row ? kBlockM : span) * BN * 2);
     }
 
-    // shared memory: operand ring (at least as large as the fp32 staging tile it becomes), residual boxes, bias2 rows,
-    // barriers, per-column vectors, per-row statistics, alignment slack
+    {
+        // the output tile's (TW, TH, TN) box over the output window, in boxes of 32 columns (64B swizzle), or of 16
+        // (32B swizzle) when the tile width is an odd multiple of 16, so that no box reaches into the next tile's columns
+        // columns past a multiple of 8 are left to the kernel's threads (a TMA store writes whole 16-byte chunks)
+        const int width = geglu ? BN / 2 : BN;
+        p.out_box_lg = width % 32 == 0 ? 5 : 4;
+        p.out_cols = geglu ? d->n_cols / 2 : d->n_cols;
+        p.out_tma_cols = p.out_cols & ~7;
+        if (p.out_tma_cols > 0) {
+            const uint64_t ldc = (uint64_t)d->ldc;
+            uint64_t dims[4] = {(uint64_t)p.out_tma_cols, (uint64_t)d->oW, (uint64_t)d->oH, (uint64_t)d->oN};
+            uint64_t strides[3] = {ldc * 2, ldc * d->oW * 2, ldc * d->oW * d->oH * 2};
+            uint32_t box[4] = {1u << p.out_box_lg, (uint32_t)p.TW, (uint32_t)p.TH, (uint32_t)p.TN};
+            const CUtensorMap* m = get_tensor_map(d->out, 4, dims, strides, box, 2 << p.out_box_lg);
+            if (!m) return TC_ERR_CUDA;
+            p.tmO = *m;
+        }
+    }
+
+    // shared memory: operand ring, residual boxes, bias2 rows, barriers, per-column vectors, per-row statistics,
+    // alignment slack.  The drained ring holds the fp16 output tile (128 x BN x 2 bytes), which two stages always exceed
     const int stage_bytes = kAStageBytes + (int)p.b_bytes;
-    const int staging_bytes = kBlockM * (BNp + 4) * 4;
     const int kFixedSmem = 1024 + 8 * (2 * 8 + 1) + 2048 + 1024 + 1024 + 64;
     const int operand_smem = (int)(p.res_smem + p.b2_smem);
     const int smem_budget = 227 * 1024 - kFixedSmem - operand_smem;
@@ -698,7 +790,7 @@ extern "C" int tc_conv_gemm(const TcConvGemm* d, void* stream_v) {
     if (stages > 8) stages = 8;
     if (stages < 2) return fail(TC_ERR_INVALID, "tc_conv_gemm: not enough shared memory for 2 stages");
     p.stages = stages;
-    const int ring = stages * stage_bytes > staging_bytes ? stages * stage_bytes : staging_bytes;
+    const int ring = stages * stage_bytes;
     p.ring_bytes = (uint32_t)ring;
     const size_t smem_bytes = (size_t)ring + operand_smem + kFixedSmem;
     TC_CHECK_ARG(smem_bytes <= 227 * 1024, "tc_conv_gemm: tile does not fit in shared memory");

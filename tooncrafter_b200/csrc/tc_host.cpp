@@ -112,7 +112,9 @@ const CUtensorMap* get_tensor_map(const void* base, int rank, const uint64_t* di
     for (int i = 0; i + 1 < rank; ++i) gstr[i] = strides_bytes[i];
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(base), gdim, gstr, bx,
                      es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                     swizzle_bytes == 32   ? CU_TENSOR_MAP_SWIZZLE_32B
+                     : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                           : CU_TENSOR_MAP_SWIZZLE_128B,
                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) {

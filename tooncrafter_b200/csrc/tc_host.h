@@ -17,7 +17,7 @@ int check_cuda(cudaError_t e, const char* what);
 void count_launch(int n = 1);
 int sm_count();
 
-// Cached cuTensorMapEncodeTiled: fp16 tensor of `rank` dims (dim 0 contiguous), 128B (or 64B) swizzle,
+// Cached cuTensorMapEncodeTiled: fp16 tensor of `rank` dims (dim 0 contiguous), 128B (or 64B / 32B) swizzle,
 // zero fill out of bounds.  strides are in BYTES for dims 1..rank-1.
 const CUtensorMap* get_tensor_map(const void* base, int rank, const uint64_t* dims, const uint64_t* strides_bytes,
                                   const uint32_t* box, int swizzle_bytes = 128);
