@@ -241,6 +241,17 @@ int tc_ddim_step(const void* e_c, const void* e_uc, const float* x, const float*
 int tc_ddim_step3(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
                   float* x_prev, float* pred_x0, const float* coef, int B, long long n, double* ws, void* stream);
 
+/* DPM-Solver++(2M) step: tc_ddim_step / tc_ddim_step3 (e_img NULL / not NULL) plus the second-order correction
+ *   x_prev += c * (pred_x0 - prev_pred_x0)     (fp32, each op rounded on its own)
+ * prev_pred_x0: the previous step's pred_x0, fp32 [B][n], a buffer other than pred_x0 (the caller swaps the two each
+ * step).  c = coef[8] (tc_dpm_step) or coef[9] (tc_dpm_step3, after cfg_img).  c == 0 is a first-order step: the
+ * result is the DDIM step's bit for bit and prev_pred_x0 is not read. */
+int tc_dpm_step(const void* e_c, const void* e_uc, const float* x, const float* noise, const float* prev_pred_x0,
+                float* x_prev, float* pred_x0, const float* coef, int B, long long n, double* ws, void* stream);
+int tc_dpm_step3(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
+                 const float* prev_pred_x0, float* x_prev, float* pred_x0, const float* coef, int B, long long n,
+                 double* ws, void* stream);
+
 /* Forward diffusion of a clean latent, in place on x (fp32 [B][n]); row b takes a = coef[2b], c = coef[2b+1]:
  *   q = clean ? x0 : a*x0 + c*noise        (q_sample / stochastic_encode: ddpm3d.py:306-309, ddim.py:309-318)
  *   x = mask ? q*m + (1 - m)*x : q         (the masked step blend of ddim.py:172-180)

@@ -106,6 +106,10 @@ _PROTOTYPES = {
                                C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
     "tc_ddim_step3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "tc_dpm_step": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
+    "tc_dpm_step3": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p]),
     "tc_q_sample": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                               C.c_longlong, C.c_void_p]),
 }

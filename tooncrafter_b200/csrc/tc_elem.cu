@@ -309,11 +309,15 @@ __global__ void ddim_reduce_kernel(const __half* __restrict__ e_c, const __half*
     }
 }
 
+// kDpm (DPM-Solver++(2M), prev_pred_x0 = the previous step's pred_x0): x_prev += c * (pred_x0 - prev_pred_x0), with
+// c = coef[8] (coef[9] with e_img) and each op rounded on its own as torch's fp32 arithmetic.  c == 0 marks a first-order
+// step: the term is skipped and prev_pred_x0 is not read.  Without kDpm this is the DDIM update, and prev_pred_x0 unused.
+template <bool kDpm>
 __global__ void ddim_update_kernel(const __half* __restrict__ e_c, const __half* __restrict__ e_uc,
                                    const __half* __restrict__ e_img, const float* __restrict__ x, const float* __restrict__ noise,
                                    float* __restrict__ x_prev, float* __restrict__ pred_x0,
                                    const float* __restrict__ coef, long long n, const double* __restrict__ ws,
-                                   int nblk) {
+                                   int nblk, const float* __restrict__ prev_pred_x0) {
     tc::pdl_wait();   // no early launch_dependents: waiting successor CTAs would squat on this kernel's SM slots
     const int b = blockIdx.y;
     const float s = coef[0], phi = coef[1], sqrt_ac = coef[2], sqrt_1mac = coef[3], rescale = coef[4],
@@ -339,6 +343,7 @@ __global__ void ddim_update_kernel(const __half* __restrict__ e_c, const __half*
     const float ratio = s_ratio;
     const long long off = (long long)b * n;
     const float cfg_img = e_img ? coef[8] : 0.f;
+    const float c2 = kDpm ? coef[e_img ? 9 : 8] : 0.f;
     const __half* ei = e_img ? e_img + off : nullptr;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
          i += (long long)gridDim.x * blockDim.x) {
@@ -355,7 +360,9 @@ __global__ void ddim_update_kernel(const __half* __restrict__ e_c, const __half*
         float x0 = sqrt_ac * xv - sqrt_1mac * v;
         x0 *= rescale;
         pred_x0[off + i] = x0;
-        x_prev[off + i] = sqrt_aprev * x0 + dir_coef * eps + sigma * noise[off + i];
+        float xp = sqrt_aprev * x0 + dir_coef * eps + sigma * noise[off + i];
+        if (kDpm && c2 != 0.f) xp = __fadd_rn(xp, __fmul_rn(c2, __fsub_rn(x0, prev_pred_x0[off + i])));
+        x_prev[off + i] = xp;
     }
 }
 
@@ -613,16 +620,17 @@ extern "C" int tc_q_sample(float* x, const float* x0, const float* noise, const 
 }
 
 static int ddim_step_impl(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
-                          float* x_prev, float* pred_x0, const float* coef, int B, long long n, double* ws,
-                          cudaStream_t stream) {
+                          const float* prev_pred_x0, float* x_prev, float* pred_x0, const float* coef, int B,
+                          long long n, double* ws, cudaStream_t stream) {
     const __half* ei = reinterpret_cast<const __half*>(e_img);
     tc_host::launch(ddim_reduce_kernel, dim3(dim3(TC_DDIM_PARTIALS, B)), dim3(256), 0, stream, 1,
                     reinterpret_cast<const __half*>(e_c), reinterpret_cast<const __half*>(e_uc), ei, coef, n, ws);
     count_launch();
     TC_CHECK_LAUNCH("ddim_reduce_kernel");
     int g = grid_for(n, 256, 4 * sm_count());
-    tc_host::launch(ddim_update_kernel, dim3(dim3(g, B)), dim3(256), 0, stream, 1, reinterpret_cast<const __half*>(e_c),
-                    reinterpret_cast<const __half*>(e_uc), ei, x, noise, x_prev, pred_x0, coef, n, ws, TC_DDIM_PARTIALS);
+    tc_host::launch(prev_pred_x0 ? ddim_update_kernel<true> : ddim_update_kernel<false>, dim3(dim3(g, B)), dim3(256), 0,
+                    stream, 1, reinterpret_cast<const __half*>(e_c), reinterpret_cast<const __half*>(e_uc), ei, x, noise,
+                    x_prev, pred_x0, coef, n, ws, TC_DDIM_PARTIALS, prev_pred_x0);
     count_launch();
     TC_CHECK_LAUNCH("ddim_update_kernel");
     return TC_OK;
@@ -632,7 +640,8 @@ extern "C" int tc_ddim_step(const void* e_c, const void* e_uc, const float* x, c
                             float* pred_x0, const float* coef, int B, long long n, double* ws, void* stream_v) {
     TC_CHECK_ARG(e_c && e_uc && x && noise && x_prev && pred_x0 && coef && ws && B > 0 && n > 1,
                  "tc_ddim_step: bad arguments");
-    return ddim_step_impl(e_c, e_uc, nullptr, x, noise, x_prev, pred_x0, coef, B, n, ws, reinterpret_cast<cudaStream_t>(stream_v));
+    return ddim_step_impl(e_c, e_uc, nullptr, x, noise, nullptr, x_prev, pred_x0, coef, B, n, ws,
+                          reinterpret_cast<cudaStream_t>(stream_v));
 }
 
 extern "C" int tc_ddim_step3(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
@@ -640,5 +649,24 @@ extern "C" int tc_ddim_step3(const void* e_c, const void* e_uc, const void* e_im
                              void* stream_v) {
     TC_CHECK_ARG(e_c && e_uc && e_img && x && noise && x_prev && pred_x0 && coef && ws && B > 0 && n > 1,
                  "tc_ddim_step3: bad arguments");
-    return ddim_step_impl(e_c, e_uc, e_img, x, noise, x_prev, pred_x0, coef, B, n, ws, reinterpret_cast<cudaStream_t>(stream_v));
+    return ddim_step_impl(e_c, e_uc, e_img, x, noise, nullptr, x_prev, pred_x0, coef, B, n, ws,
+                          reinterpret_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int tc_dpm_step(const void* e_c, const void* e_uc, const float* x, const float* noise,
+                           const float* prev_pred_x0, float* x_prev, float* pred_x0, const float* coef, int B,
+                           long long n, double* ws, void* stream_v) {
+    TC_CHECK_ARG(e_c && e_uc && x && noise && prev_pred_x0 && x_prev && pred_x0 && coef && ws && B > 0 && n > 1 &&
+                 prev_pred_x0 != pred_x0, "tc_dpm_step: bad arguments");
+    return ddim_step_impl(e_c, e_uc, nullptr, x, noise, prev_pred_x0, x_prev, pred_x0, coef, B, n, ws,
+                          reinterpret_cast<cudaStream_t>(stream_v));
+}
+
+extern "C" int tc_dpm_step3(const void* e_c, const void* e_uc, const void* e_img, const float* x, const float* noise,
+                            const float* prev_pred_x0, float* x_prev, float* pred_x0, const float* coef, int B,
+                            long long n, double* ws, void* stream_v) {
+    TC_CHECK_ARG(e_c && e_uc && e_img && x && noise && prev_pred_x0 && x_prev && pred_x0 && coef && ws && B > 0 &&
+                 n > 1 && prev_pred_x0 != pred_x0, "tc_dpm_step3: bad arguments");
+    return ddim_step_impl(e_c, e_uc, e_img, x, noise, prev_pred_x0, x_prev, pred_x0, coef, B, n, ws,
+                          reinterpret_cast<cudaStream_t>(stream_v));
 }

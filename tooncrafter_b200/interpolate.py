@@ -92,6 +92,8 @@ def get_parser() -> argparse.ArgumentParser:
     ap.add_argument("--width", type=int, default=512)
     ap.add_argument("--ddim-steps", type=int, default=50)
     ap.add_argument("--ddim-eta", type=float, default=1.0)
+    ap.add_argument("--sampler", default="ddim",
+                    help="ddim (the reference's sampler) or dpmpp_2m (DPM-Solver++(2M), --ddim-eta 0 or 1)")
     ap.add_argument("--cfg-scale", type=float, default=7.5, help="classifier-free guidance scale")
     ap.add_argument("--cfg-img", type=float, default=None, help="image guidance scale (three-way guidance)")
     ap.add_argument("--frame-stride", type=int, default=10, help="fs conditioning (smaller: larger motion)")
@@ -276,7 +278,9 @@ def main(argv=None) -> int:
     if args.frames is None and args.prompt_dir is None and args.init_video is None:
         ap.error("one of the arguments --frames --prompt-dir is required (or --init-video to refine a clip)")
     from .pipeline import check_count, check_n_samples, check_strength, check_video_length
+    from .sampler import check_sampler
     try:
+        check_sampler(args.sampler, args.ddim_eta)
         if args.video_length is not None:
             check_video_length(args.video_length)
         if args.n_samples is not None:
@@ -351,7 +355,7 @@ def run(args, cfg, dev, group) -> int:
     pipe = ToonCrafterPipeline(model, group, latency=args.latency_mode)
     common = dict(steps=args.ddim_steps, cfg_scale=args.cfg_scale, eta=args.ddim_eta, fs=args.frame_stride,
                   guidance_rescale=args.guidance_rescale, timestep_spacing=args.timestep_spacing, cfg_img=args.cfg_img,
-                  size=(args.height, args.width), video_length=args.video_length)
+                  size=(args.height, args.width), video_length=args.video_length, sampler=args.sampler)
     writes = group is None or torch.distributed.get_rank() == 0
     if args.prompt_dir is not None:
         return run_prompt_dir(args, pipe, common, group, writes)

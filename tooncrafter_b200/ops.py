@@ -339,6 +339,23 @@ def ddim_step3(e_c, e_uc, e_img, x, noise, x_prev, pred_x0, coef, ws, *, B: int,
           "tc_ddim_step3")
 
 
+def dpm_step(e_c, e_uc, x, noise, prev_pred_x0, x_prev, pred_x0, coef, ws, *, B: int, n: int) -> None:
+    """ddim_step plus DPM-Solver++(2M)'s correction x_prev += coef[8] * (pred_x0 - prev_pred_x0); coef holds 9 floats.
+    prev_pred_x0 (the previous step's pred_x0) must be a buffer other than pred_x0; coef[8] == 0 leaves it unread."""
+    lib = _lib.load()
+    check(lib.tc_dpm_step(e_c.data_ptr(), e_uc.data_ptr(), x.data_ptr(), noise.data_ptr(), prev_pred_x0.data_ptr(),
+                          x_prev.data_ptr(), pred_x0.data_ptr(), coef.data_ptr(), B, n, ws.data_ptr(), _stream()),
+          "tc_dpm_step")
+
+
+def dpm_step3(e_c, e_uc, e_img, x, noise, prev_pred_x0, x_prev, pred_x0, coef, ws, *, B: int, n: int) -> None:
+    """ddim_step3 plus the correction of dpm_step, whose weight is coef[9] (after cfg_img); coef holds 10 floats."""
+    lib = _lib.load()
+    check(lib.tc_dpm_step3(e_c.data_ptr(), e_uc.data_ptr(), e_img.data_ptr(), x.data_ptr(), noise.data_ptr(),
+                           prev_pred_x0.data_ptr(), x_prev.data_ptr(), pred_x0.data_ptr(), coef.data_ptr(), B, n,
+                           ws.data_ptr(), _stream()), "tc_dpm_step3")
+
+
 def q_sample(x, x0, noise, mask, coef, *, B: int, n: int, clean: bool = False) -> None:
     """In place on x (fp32 [B][n]): q = x0 if clean else coef[2b]*x0 + coef[2b+1]*noise per row b, then x = q where
     mask is None, else q*mask + (1 - mask)*x.  torch's fp32 op order, bit for bit.  x0 / noise / mask: contiguous fp32

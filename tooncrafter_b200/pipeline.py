@@ -73,7 +73,7 @@ import torch.distributed as dist
 
 from . import distributed, ops, runtime
 from .modules import VideoDecoder, clip_tokenize
-from .sampler import DDIMSampler, DDIMSamplerMultiCond, randn_rows
+from .sampler import SAMPLERS, check_sampler, randn_rows
 
 
 def preprocess(keyframes, size=(320, 512), device="cpu") -> torch.Tensor:
@@ -182,6 +182,7 @@ class _Call(NamedTuple):
     guidance_rescale: float
     timestep_spacing: str
     cfg_img: Optional[float]
+    sampler: str                # a key of sampler.SAMPLERS
 
 
 class _Row(NamedTuple):
@@ -270,7 +271,8 @@ class ToonCrafterPipeline:
                     cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                     timestep_spacing: str = "uniform_trailing", cfg_img=None, loop: bool = False, seed: int = 123,
                     size=(320, 512), segments_per_batch: Optional[int] = None, output: str = "uint8",
-                    video_length: Optional[int] = None, n_samples: Optional[int] = None) -> torch.Tensor:
+                    video_length: Optional[int] = None, n_samples: Optional[int] = None,
+                    sampler: str = "ddim") -> torch.Tensor:
         """keyframes: K >= 2 uint8 RGB images (tensor [K, H, W, 3], ndarray, or a list of [H, W, 3] arrays of any
         size).  prompts: one string for every segment, a list of S strings, or token ids [S, 77] (strings other than
         "" need open_clip's tokenizer).  cfg_img not None: three-way guidance (DDIMSamplerMultiCond).  Defaults are
@@ -285,9 +287,13 @@ class ToonCrafterPipeline:
         Returns uint8 [F, size[0], size[1], 3] on the model's device, F = (T-1)*S + 1 (or (T-1)*K with `loop`); with
         output="float", the spliced per-segment videos before quantisation, float32 [S, 3, T, size[0], size[1]].
         With an integer n_samples both gain a leading variant axis, [n, F, H, W, 3] / [n, S, 3, T, H, W], and
-        video[v] is a complete single-sample result (video[0] is the n_samples=None result)."""
+        video[v] is a complete single-sample result (video[0] is the n_samples=None result).
+
+        sampler: "ddim" (the reference's sampler) or "dpmpp_2m" (DPM-Solver++(2M), eta 0 or 1: the same UNet
+        evaluations per step, second order; INTEGRATION.md).  Every method takes it; ValueError for an unknown name or
+        dpmpp_2m with another eta, before any work."""
         c = self._checked(video_length, n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
-                          guidance_rescale, timestep_spacing, cfg_img)
+                          guidance_rescale, timestep_spacing, cfg_img, sampler)
         frames = preprocess(keyframes, c.size, self.model.device)
         K = frames.shape[0]
         if K < 2:
@@ -300,7 +306,7 @@ class ToonCrafterPipeline:
                 eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                 timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
                 output: str = "uint8", video_length: Optional[int] = None, n_samples: Optional[int] = None,
-                segments_per_batch: Optional[int] = None) -> torch.Tensor:
+                segments_per_batch: Optional[int] = None, sampler: str = "ddim") -> torch.Tensor:
         """One image -> one T-frame video: image_guided_synthesis with interp=False, loop=False (inference.py:
         180-277; c_concat is the image's latent repeated over the T frames, :201-203), the image-to-video mode of
         the DynamiCrafter checkpoints.  image: a uint8 [H, W, 3] RGB image of any size; prompt: a string or token
@@ -310,9 +316,10 @@ class ToonCrafterPipeline:
         n_samples / segments_per_batch (variants sampled per call), as for interpolate.
 
         Returns uint8 [T, size[0], size[1], 3] on the model's device; with output="float", the spliced video before
-        quantisation, float32 [3, T, size[0], size[1]]; with an integer n_samples, [n, T, H, W, 3] / [n, 3, T, H, W]."""
+        quantisation, float32 [3, T, size[0], size[1]]; with an integer n_samples, [n, T, H, W, 3] / [n, 3, T, H, W].
+        sampler: as for interpolate."""
         c = self._checked(video_length, n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
-                          guidance_rescale, timestep_spacing, cfg_img)
+                          guidance_rescale, timestep_spacing, cfg_img, sampler)
         frames = preprocess([image], c.size, self.model.device)
         return self._generate(frames, prompt, [0], [0], False, False, seed, c, segment_axis=False)
 
@@ -321,7 +328,7 @@ class ToonCrafterPipeline:
                steps: int = 50, cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10, guidance_rescale: float = 0.7,
                timestep_spacing: str = "uniform_trailing", cfg_img=None, seed: int = 123, size=(320, 512),
                output: str = "uint8", n_samples: Optional[int] = None,
-               segments_per_batch: Optional[int] = None) -> torch.Tensor:
+               segments_per_batch: Optional[int] = None, sampler: str = "ddim") -> torch.Tensor:
         """Re-render an existing clip (SDEdit: DDIMSampler.stochastic_encode, then the last k DDIM steps), conditioned
         on its own first and last frames exactly as interpolate([clip[0], clip[T-1]], video_length=T) is.
 
@@ -342,9 +349,10 @@ class ToonCrafterPipeline:
 
         Returns what a one-segment interpolate returns: uint8 [T, size[0], size[1], 3], or float32 [3, T, size[0],
         size[1]] with output="float"; an integer n_samples adds a leading variant axis.  ValueError for a bad clip
-        length, strength, keep, n_samples, segments_per_batch or output before any work."""
+        length, strength, keep, n_samples, segments_per_batch, output or sampler before any work.  sampler: as for
+        interpolate; the last k steps run with it."""
         c = self._checked(len(clip), n_samples, segments_per_batch, size, output, steps, cfg_scale, eta, fs,
-                          guidance_rescale, timestep_spacing, cfg_img)
+                          guidance_rescale, timestep_spacing, cfg_img, sampler)
         T = c.T
         k, keep = check_strength(strength, steps), check_keep(keep, T)
         frames = preprocess(clip, c.size, self.model.device)
@@ -357,7 +365,8 @@ class ToonCrafterPipeline:
                           steps: int = 50, cfg_scale: float = 7.5, eta: float = 1.0, fs: int = 10,
                           guidance_rescale: float = 0.7, timestep_spacing: str = "uniform_trailing", cfg_img=None,
                           seed: int = 123, size=(320, 512), pairs_per_batch: Optional[int] = None,
-                          output: str = "uint8", video_length: Optional[int] = None) -> torch.Tensor:
+                          output: str = "uint8", video_length: Optional[int] = None,
+                          sampler: str = "ddim") -> torch.Tensor:
         """P independent keyframe pairs -> n_samples T-frame clips each: the reference's --prompt_dir --interp run
         (module docstring).  pairs: P pairs of uint8 RGB images (a sequence of (a, b), or a tensor [P, 2, H, W, 3]);
         prompts: one string for every pair, a list of P strings, or token ids [P, 77].
@@ -368,13 +377,13 @@ class ToonCrafterPipeline:
         per sample() call); None: default_pairs_per_batch(size, T, n).
 
         Returns uint8 [P, n, T, size[0], size[1], 3] on the model's device, every pair's whole clip; with
-        output="float", float32 [P, n, 3, T, size[0], size[1]]."""
+        output="float", float32 [P, n, 3, T, size[0], size[1]].  sampler: as for interpolate."""
         P = len(pairs)
         if P < 1 or any(len(p) != 2 for p in pairs):
             raise ValueError("pairs must be a non-empty sequence of (image, image) pairs")
         _check_prompts(prompts, P, "pairs")
         c = self._checked(video_length, n_samples, pairs_per_batch, size, output, steps, cfg_scale, eta, fs,
-                          guidance_rescale, timestep_spacing, cfg_img, pairs=True)
+                          guidance_rescale, timestep_spacing, cfg_img, sampler, pairs=True)
         n, T = c.n, c.T
         # pair-major rows: pair i's variant v is row i * n + v, its whole clip (frames 0 .. T-1, no seam)
         rows = [_Row(i, seed + i + v * VARIANT_SEED_STRIDE, i * n + v, 0, T, (i * n + v) * T)
@@ -394,7 +403,7 @@ class ToonCrafterPipeline:
         return (video.view(P, n, T, *c.size, 3) if c.output == "uint8" else video.view(P, n, 3, T, *c.size))
 
     def _checked(self, video_length, n_samples, per_batch, size, output, steps, cfg_scale, eta, fs, guidance_rescale,
-                 timestep_spacing, cfg_img, pairs: bool = False) -> _Call:
+                 timestep_spacing, cfg_img, sampler, pairs: bool = False) -> _Call:
         """The argument checks the public methods share, all before any work; returns the normalised arguments.
         video_length None: the model's temporal_length.  per_batch: segments_per_batch, or pairs_per_batch with
         `pairs` (where n_samples must be an integer); None: its default."""
@@ -406,6 +415,7 @@ class ToonCrafterPipeline:
             per_batch = default_pairs_per_batch(size, T, n) if pairs else default_segments_per_batch(size, T)
         if output not in ("uint8", "float"):
             raise ValueError(f"output must be 'uint8' or 'float', got {output!r}")
+        check_sampler(sampler, eta)
         if size[0] % 16 or size[1] % 16:
             raise ValueError(f"size {tuple(size)} must be a multiple of 16")
         if self.model.model.conditioning_key != "hybrid":
@@ -417,7 +427,7 @@ class ToonCrafterPipeline:
             raise ValueError("latency mode splits the conditional and unconditional branches over a GPU pair; "
                              "cfg_scale 1.0 has no unconditional branch")
         return _Call(T, n, per_batch, pairs or n_samples is not None, tuple(size), output, steps, cfg_scale, eta, fs,
-                     guidance_rescale, timestep_spacing, cfg_img)
+                     guidance_rescale, timestep_spacing, cfg_img, sampler)
 
     def _mine(self, n_items: int):
         """The items (rows, pairs) of this rank's block: all of them without a group."""
@@ -489,7 +499,8 @@ class ToonCrafterPipeline:
             c_concat = z[first][:, :, None].expand(-1, -1, T, -1, -1).contiguous()
         x0 = None if refine is None else self._clip_latents(z, refine.frames, refine.seeds)   # [1, 4, T, h, w]
 
-        sampler = DDIMSampler(m) if c.cfg_img is None else DDIMSamplerMultiCond(m)
+        two_way, three_way = SAMPLERS[c.sampler]
+        sampler = two_way(m) if c.cfg_img is None else three_way(m)
         sampler.latency_group = self._pair
         decodes = not (self.latency and self._pair_rank)          # in a latency pair, pair-rank 0 decodes
         dec = m.first_stage_model.decoder_engine() if decodes else None

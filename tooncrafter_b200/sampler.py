@@ -317,20 +317,29 @@ class DDIMSampler(object):
         if len(extra_branches) > 1 or (extra_branches and group is not None):
             raise NotImplementedError("fused path: at most one extra guidance branch, not in latency mode")
         tail = [float(cfg_img)] if st.three else []
-        st.q_off = 8 + len(tail)
+        order2 = self._order2_coefficients([index for index, _ in steps])
+        st.order2 = order2 is not None
+        st.q_off = 8 + len(tail) + st.order2
         q = lambda t: ([float(m.sqrt_alphas_cumprod[t]), float(m.sqrt_one_minus_alphas_cumprod[t])] * b
                        if q_coefficients else [])
-        st.coef_table = torch.tensor([self.step_coefficients(index, cfg_scale, phi, temperature) + tail + q(int(t))
-                                      for index, t in steps], dtype=torch.float32, device=dev)
+        c2 = lambda i: [order2[i]] if st.order2 else []
+        st.coef_table = torch.tensor([self.step_coefficients(index, cfg_scale, phi, temperature) + tail + c2(i) +
+                                      q(int(t)) for i, (index, t) in enumerate(steps)], dtype=torch.float32, device=dev)
         st.t_table = torch.tensor([float(t) for _, t in steps], dtype=torch.float32, device=dev)
         st.ws = torch.empty(4 * b * ops.DDIM_PARTIALS, dtype=torch.float64, device=dev)
         if group is not None:
             st.e_all = torch.empty((2 * b,) + tuple(plan.y_out.shape[1:]), dtype=plan.y_out.dtype, device=dev)
         return st
 
-    def _fused_step(self, st, i, x, noise, x_next, pred_x0):
+    def _order2_coefficients(self, indices):
+        """None for DDIM; a second-order sampler returns the weight of its correction term for each step of `indices`
+        (DDIM indices in execution order), which the fused update reads from the table column after cfg_img."""
+        return None
+
+    def _fused_step(self, st, i, x, noise, x_next, pred_x0, prev_pred_x0=None):
         """One DDIM step (row i of the tables): batched UNet program replay + the fused update.  Writes x_next and
-        pred_x0; afterwards st.plan.y_out still holds the two UNet predictions of this step."""
+        pred_x0; afterwards st.plan.y_out still holds the two UNet predictions of this step.  prev_pred_x0: the previous
+        step's pred_x0, read by the second-order update (st.order2)."""
         plan, b, c = st.plan, st.b, st.c
         for r in range(st.nb // b):                                          # the same latent under every branch
             plan.x_in[r * b:(r + 1) * b, :c].copy_(x)
@@ -346,8 +355,14 @@ class DDIMSampler(object):
             from .distributed import pair_all_gather
             pair_all_gather(st.e_all, plan.y_out, st.group)                      # the step's only exchange (2 x 327 KB)
             e_c, e_uc = st.e_all[:b], st.e_all[b:]
-        fn, args = ((ops.ddim_step3, (e_c, e_uc, e_img, x, noise, x_next, pred_x0, st.coef_table[i], st.ws)) if st.three
-                    else (ops.ddim_step, (e_c, e_uc, x, noise, x_next, pred_x0, st.coef_table[i], st.ws)))
+        if st.order2:
+            fn, args = ((ops.dpm_step3, (e_c, e_uc, e_img, x, noise, prev_pred_x0, x_next, pred_x0, st.coef_table[i],
+                                         st.ws)) if st.three
+                        else (ops.dpm_step, (e_c, e_uc, x, noise, prev_pred_x0, x_next, pred_x0, st.coef_table[i],
+                                             st.ws)))
+        else:
+            fn, args = ((ops.ddim_step3, (e_c, e_uc, e_img, x, noise, x_next, pred_x0, st.coef_table[i], st.ws))
+                        if st.three else (ops.ddim_step, (e_c, e_uc, x, noise, x_next, pred_x0, st.coef_table[i], st.ws)))
         if st.ex is None:
             fn(*args, B=b, n=st.n)
         else:
@@ -363,6 +378,8 @@ class DDIMSampler(object):
         x = img.to(torch.float32).contiguous().clone()
         x_next = torch.empty_like(x)
         pred_x0 = torch.empty_like(x)
+        # second order: the update reads the previous step's pred_x0 from one buffer and writes into the other
+        prev_pred_x0 = torch.zeros_like(x) if st.order2 else None
         if mask is not None:
             assert x0 is not None
             # expanded once per call; the blend is then one tc_q_sample launch per step
@@ -383,7 +400,9 @@ class DDIMSampler(object):
                 else:
                     st.ex(ops.q_sample, args, kw)
             noise = randn_rows(x.shape, st.dev, noise_generators)          # one draw per step, as ddim.py:273
-            self._fused_step(st, i, x, noise, x_next, pred_x0)
+            if prev_pred_x0 is not None:
+                pred_x0, prev_pred_x0 = prev_pred_x0, pred_x0
+            self._fused_step(st, i, x, noise, x_next, pred_x0, prev_pred_x0)
             x, x_next = x_next, x
             if callback:
                 callback(i)
@@ -493,3 +512,85 @@ class DDIMSamplerMultiCond(DDIMSampler):
                 model_output = rescale_noise_cfg(model_output, e_c, guidance_rescale=guidance_rescale)
         return self._ddim_update(x, t, index, model_output, c, repeat_noise, use_original_steps, quantize_denoised,
                                  temperature, noise_dropout, score_corrector, corrector_kwargs, noise_generators)
+
+
+def check_dpm_eta(eta) -> float:
+    """DPM-Solver++(2M) is defined for eta 0 (the ODE solver) and eta 1 (its SDE form): its first-order step is the DDIM
+    step with that eta, and no other eta has such a counterpart."""
+    if isinstance(eta, bool) or eta not in (0, 1):
+        raise ValueError(f"DPM-Solver++(2M) takes eta 0 or 1, got {eta!r}")
+    return float(eta)
+
+
+class _DPMSolverPP2M:
+    """DPM-Solver++(2M) in data-prediction form, as the DDIM step plus one correction (INTEGRATION.md):
+
+        x' = DDIM_eta(x, p_i) + c_i * (p_i - p_{i-1}),   p_i = pred_x0 of step i (after the dynamic rescale)
+
+    With a = ddim_alphas[index], a' = ddim_alphas_prev[index], alpha = sqrt(a), sigma = sqrt(1 - a),
+    lambda = log(alpha / sigma) and h_i = lambda' - lambda:  c_i = alpha' (1 - e^{-h_i}) / (2 r_i) for eta 0,
+    alpha' (1 - e^{-2 h_i}) / (2 r_i) for eta 1, with r_i = h_{i-1} / h_i.  c_i = 0 (a DDIM step) on the first step that
+    runs and on a step whose predecessor started at lambda = -inf (zero terminal SNR).  The noise draws are DDIM's, so
+    either sampler consumes a generator's stream alike.  Works on the fused path (tc_dpm_step*) and the general path."""
+
+    def make_schedule(self, ddim_num_steps, ddim_discretize="uniform", ddim_eta=0.0, verbose=True):
+        self.dpm_eta = check_dpm_eta(ddim_eta)
+        super().make_schedule(ddim_num_steps, ddim_discretize, ddim_eta, verbose)
+
+    def order2_weights(self) -> np.ndarray:
+        """float64 [S] of the last make_schedule: entry k is c of a step at DDIM index k whose predecessor ran at index
+        k + 1; 0 for index S - 1 and wherever that predecessor has alpha = 0.  Always finite."""
+        a = self.ddim_alphas.detach().double().cpu().numpy()
+        ap = np.asarray(self.ddim_alphas_prev, dtype=np.float64)
+        al, sg, alp, sgp = np.sqrt(a), np.sqrt(1.0 - a), np.sqrt(ap), np.sqrt(1.0 - ap)
+        with np.errstate(divide="ignore"):
+            h = np.log((alp * sg) / (sgp * al))                     # lambda' - lambda; inf where alpha = 0
+        e_mh = (al * sgp) / (sg * alp)                               # e^{-h}, as the ratio
+        w = 1.0 - (e_mh if self.dpm_eta == 0.0 else e_mh * e_mh)
+        c = np.zeros(a.shape[0])
+        for k in range(a.shape[0] - 1):
+            if al[k + 1] > 0.0:
+                c[k] = alp[k] * w[k] / (2.0 * (h[k + 1] / h[k]))
+        return c
+
+    def _order2_coefficients(self, indices):
+        w = self.order2_weights()
+        return [0.0] + [float(w[k]) for k in indices[1:]]
+
+    @torch.no_grad()
+    def ddim_sampling(self, cond, shape, x_T=None, ddim_use_original_steps=False, **kwargs):
+        if ddim_use_original_steps:
+            raise NotImplementedError("DPM-Solver++(2M) runs on the DDIM schedule, not the original DDPM steps")
+        self._order2_w = self.order2_weights()
+        self._prev_pred_x0 = None                        # the general path's p_{i-1}; None: the next step is first order
+        return super().ddim_sampling(cond, shape, x_T=x_T, ddim_use_original_steps=False, **kwargs)
+
+    def _ddim_update(self, x, t, index, *args, **kwargs):
+        """The general path: DDIM's update in torch, then the correction in fp32, one rounding per op (as tc_dpm_step)."""
+        x_prev, pred_x0 = super()._ddim_update(x, t, index, *args, **kwargs)
+        prev, self._prev_pred_x0 = self._prev_pred_x0, pred_x0
+        c = float(np.float32(self._order2_w[index])) if prev is not None else 0.0
+        if c != 0.0:
+            x_prev = x_prev + c * (pred_x0 - prev)
+        return x_prev, pred_x0
+
+
+class DPMSolverSampler(_DPMSolverPP2M, DDIMSampler):
+    """DDIMSampler's interface (sample, stochastic_encode, decode, noise_generators, t_start, mask / x0, latency_group)
+    with DPM-Solver++(2M) steps; eta must be 0 or 1."""
+
+
+class DPMSolverSamplerMultiCond(_DPMSolverPP2M, DDIMSamplerMultiCond):
+    """DDIMSamplerMultiCond's three-way guidance (cfg_img) with DPM-Solver++(2M) steps; eta must be 0 or 1."""
+
+
+SAMPLERS = {"ddim": (DDIMSampler, DDIMSamplerMultiCond), "dpmpp_2m": (DPMSolverSampler, DPMSolverSamplerMultiCond)}
+
+
+def check_sampler(name, eta) -> str:
+    """A key of SAMPLERS, with an eta that sampler takes (dpmpp_2m: 0 or 1); ValueError otherwise."""
+    if name not in SAMPLERS:
+        raise ValueError(f"sampler must be one of {sorted(SAMPLERS)}, got {name!r}")
+    if name == "dpmpp_2m":
+        check_dpm_eta(eta)
+    return name
